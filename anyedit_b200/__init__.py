@@ -1,4 +1,4 @@
-"""anyedit_b200 -- B200-native AnySD denoising hot path (UNet forward + CFG/DDIM loop).
+"""anyedit_b200 -- H100-native AnySD denoising hot path (UNet forward + CFG/DDIM loop).
 
 Public surface mirrors the reference's module API for this path:
     anyedit_b200.unet.UNetModel        <- ldm.modules.diffusionmodules.openaimodel.UNetModel

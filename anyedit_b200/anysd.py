@@ -1,4 +1,4 @@
-"""AnySD task-aware router + learnable task embedding on top of the B200 UNet.
+"""AnySD task-aware router + learnable task embedding on top of the H100 UNet.
 
 The AnySD model code is absent from the reference (empty, un-pinned submodule: .gitmodules:1-4,
 SURVEY.md 0.2), so this follows the specification restated in ``oracle/anysd_oracle.py`` from the

@@ -1,4 +1,4 @@
-"""B200-native first stage: ``AutoencoderKL`` -- drop-in for ``ldm.models.autoencoder.AutoencoderKL`` (encode / decode)
+"""H100-native first stage: ``AutoencoderKL`` -- drop-in for ``ldm.models.autoencoder.AutoencoderKL`` (encode / decode)
 with the ``Encoder`` / ``Decoder`` of ``ldm.modules.diffusionmodules.model`` (SURVEY.md 8f rank 1: the step right before /
 after the denoising loop, visual_reference_tool.py:220).
 
@@ -7,7 +7,7 @@ keys and shapes (``encoder.*``, ``decoder.*``, ``quant_conv``, ``post_quant_conv
 ``encode(x) -> DiagonalGaussianDistribution``, ``decode(z) -> image``.  Execution reuses the UNet's kernels through the C ABI:
 
   ResnetBlock  (model.py:91-150)    GroupNorm(32, eps 1e-6)+swish fused -> implicit-GEMM conv3x3 (+ bias, + residual / nin_shortcut)
-  AttnBlock    (model.py:152-203)   ONE head of width C: the tcgen05 attention kernel when C <= 160; for the C = 512 of the SD
+  AttnBlock    (model.py:152-203)   ONE head of width C: the wgmma attention kernel when C <= 160; for the C = 512 of the SD
                                     autoencoder two contractions around a row softmax (S = q k^T in fp32, P fp16, O = P v)
   Downsample   (model.py:68-88)     F.pad(x, (0,1,0,1)) + conv3x3 stride 2 pad 0 = the conv kernel's right/bottom padding mode
   Upsample     (model.py:49-65)     nearest x2 + conv3x3 (the UNet's upsample conv)

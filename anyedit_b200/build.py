@@ -1,4 +1,4 @@
-"""Build the in-tree CUDA library ``anyedit_b200/libanysd_b200.so`` for sm_100a with nvcc.
+"""Build the in-tree CUDA library ``anyedit_b200/libanysd_b200.so`` for sm_90a (H100) with nvcc.
 
 No torch extension machinery: plain ``nvcc`` -> object files -> one shared library with a
 C ABI (include/anysd_b200.h), loaded through ctypes.  nvcc cross-compiles without a GPU.
@@ -14,7 +14,8 @@ CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libanysd_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+FLAGS = [*ARCH, "-O3", "-lineinfo", "-std=c++17",
          "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 
 
@@ -54,7 +55,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
 
     with ThreadPoolExecutor(max_workers=min(8, os.cpu_count() or 1)) as ex:
         objs = list(ex.map(compile_one, _sources()))
-    cmd = [NVCC, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", LIB, *objs]
+    cmd = [NVCC, "-shared", *ARCH, "-o", LIB, *objs]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

@@ -1,4 +1,4 @@
-"""ControlNet branch on the B200 kernels (SURVEY.md 8f rank 3) -- the only in-tree end-to-end consumer of the ``ldm`` UNet
+"""ControlNet branch on the H100 kernels (SURVEY.md 8f rank 3) -- the only in-tree end-to-end consumer of the ``ldm`` UNet
 (AnyDoor visual reference, AnyEdit_Collection/other_modules/cldm/cldm.py).
 
   ``ControlNet``            cldm.py:47-304: the UNet's encoder half (input blocks + middle block), a hint stem of eight 3x3
@@ -12,7 +12,7 @@
                             ``c_crossattn`` the text context, ``control_scales`` folded into the packed zero-conv weights.
 
 Execution: the hint stem's channels (16 / 32 / 96 / 256) are zero-padded to multiples of 64 so that all eight convs run on
-the tcgen05 implicit-GEMM kernel with the SiLU in the epilogue (SiLU(0) = 0 keeps the padding exact); the stem depends on
+the wgmma implicit-GEMM kernel with the SiLU in the epilogue (SiLU(0) = 0 keeps the padding exact); the stem depends on
 neither x nor t, so its output is kept for as long as the hint tensor is unchanged (a sampling run computes it once, the
 reference recomputes it every step); the residuals stay NHWC fp16 and are added to the UNet's activations by one kernel each
 (no NCHW round trip).  Two-call CFG of ``ddim_hacked.py:181-232`` = the batched [uncond ; cond] call of ``DDIMSampler``

@@ -28,12 +28,12 @@ int check_launch(const char* what) {
 int sm_count() {
     static thread_local int cached_dev = -1, cached = 0;
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return 148;
+    if (cudaGetDevice(&dev) != cudaSuccess) return 132;
     if (dev != cached_dev) {
         cudaDeviceGetAttribute(&cached, cudaDevAttrMultiProcessorCount, dev);
         cached_dev = dev;
     }
-    return cached > 0 ? cached : 148;
+    return cached > 0 ? cached : 132;
 }
 
 }  // namespace anysd

@@ -537,7 +537,7 @@ __global__ void __launch_bounds__(AB_THREADS) expert_attn_kernel(const ExpArgs p
 // of the (batch, head) are staged once -- expert e in key slots [16 e, 16 e + 16), unused slots zero -- and a 64-key tile of the
 // products covers FOUR experts: each expert's softmax is a segment of 16 columns (two n8 fragments), normalised and gated
 // before P.V, so the accumulator simply adds over all keys.  Same arithmetic per expert as above (fp32 softmax, fp16 P),
-// 3 tile passes instead of 11 for E = 11.  [measured, B = 16, 8 heads, 4096 queries, d = 40, E = 11] forward 373 -> 206 us.
+// 3 tile passes instead of 11 for E = 11.
 template <int DP, bool BWD>
 __global__ void __launch_bounds__(AB_THREADS) expert_attn16_kernel(const ExpArgs p, int groups, int qtiles) {
     constexpr int LDS = DP + 8, TILE = AB_T * LDS, CH = DP / 8;
@@ -712,9 +712,8 @@ static int launch_experts(const ExpArgs& a, const BwdArgs* dkv, int B, cudaStrea
             set16[dev] = smem16;
         }
     }
-    // query tiles per CTA: 1.  [measured, B = 16, 8 heads, 4096 queries, E = 11] 1 / 2 / 4 / 8 tiles per CTA: 1.94 / 1.96 / 1.99 /
-    // 1.98 ms per training step for the 16 forward launches -- staging the 37 KB of K/V is not what the kernel waits for (ncu: 33 %
-    // issue slots, 2.2 K instructions per warp and tile, most of them the segmented softmax).  ANYSD_EXPERT_QT overrides.
+    // query tiles per CTA: 1 (staging the 37 KB of K/V once for several query tiles did not pay on the project's earlier GPU; not
+    // re-measured on the H100).  ANYSD_EXPERT_QT overrides.
     static const char* qt_env = getenv("ANYSD_EXPERT_QT");
     const int qtiles = (use16 && qt_env && atoi(qt_env) > 0) ? atoi(qt_env) : 1;
     const dim3 grid16(cdiv(a.n_q, AB_T * qtiles), a.heads, B);
@@ -767,8 +766,8 @@ static int launch_bwd(const BwdArgs& a, int B, cudaStream_t st, bool need_dkv) {
 using namespace anysd;
 
 namespace anysd {
-bool attention_bwd_tc5_supported(const anysd_attn_bwd_params* q);
-int launch_attention_bwd_tc5(const anysd_attn_bwd_params* q, cudaStream_t st);
+bool attention_bwd_wg_supported(const anysd_attn_bwd_params* q);
+int launch_attention_bwd_wg(const anysd_attn_bwd_params* q, cudaStream_t st);
 }
 
 extern "C" size_t anysd_attention_bwd_workspace_bytes(int B, int heads, int n_q) {
@@ -801,8 +800,8 @@ extern "C" int anysd_attention_bwd_f16(const anysd_attn_bwd_params* p, anysd_str
     ANYSD_REQUIRE(p->heads <= 65535 && p->B <= 65535, ANYSD_EINVAL, "attention_bwd: grid too large");
     ANYSD_REQUIRE(p->out == nullptr || (p->gate == nullptr && p->ld_o % 8 == 0 && ((uintptr_t)p->out % 16) == 0 && p->o_batch_stride % 8 == 0),
                   ANYSD_EINVAL, "attention_bwd: `out` must be the un-gated output of this attention, 16-byte aligned, ld_o %% 8 == 0");
-    // tcgen05 kernels when the forward's log-sum-exp came along and the shape allows (attention_bwd_tc5.cu)
-    if (attention_bwd_tc5_supported(p)) return launch_attention_bwd_tc5(p, (cudaStream_t)stream);
+    // wgmma kernels when the forward's log-sum-exp came along and the shape allows (attention_wgmma.cu)
+    if (attention_bwd_wg_supported(p)) return launch_attention_bwd_wg(p, (cudaStream_t)stream);
     BwdArgs a;
     a.q = (const __half*)p->q; a.k = (const __half*)p->k; a.v = (const __half*)p->v; a.dout = (const __half*)p->d_out;
     a.dq = (__half*)p->dq; a.dk = (__half*)p->dk; a.dv = (__half*)p->dv;

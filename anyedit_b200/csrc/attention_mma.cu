@@ -11,8 +11,8 @@
 
 namespace anysd {
 
-int launch_attention_tc5(const anysd_attn_params* q, cudaStream_t st);
-bool attention_tc5_supported(const anysd_attn_params* q);
+int launch_attention_wg(const anysd_attn_params* q, cudaStream_t st);
+bool attention_wg_supported(const anysd_attn_params* q);
 
 constexpr int ATT_BQ = 64, ATT_BKV = 64, ATT_THREADS = 128;
 
@@ -253,12 +253,12 @@ extern "C" int anysd_attention_f16(const anysd_attn_params* p, anysd_stream_t st
     ANYSD_REQUIRE(p->heads <= 65535 && p->B <= 65535, ANYSD_EINVAL, "attention: grid too large");
     ANYSD_REQUIRE(p->head_stride == 0 || (p->head_stride >= p->d && p->head_stride % 8 == 0), ANYSD_EINVAL,
                   "attention: head_stride must be 0 or a multiple of 8 >= d");
-    // tcgen05 kernel whenever its layout constraints hold; ANYSD_ATTN=mma|tc5 is a test/debug switch.
+    // wgmma kernel whenever its layout constraints hold; ANYSD_ATTN=mma|wgmma is a test/debug switch.
     static const char* force = getenv("ANYSD_ATTN");
-    const bool want_tc5 = !force || !strcmp(force, "tc5");
-    if (want_tc5 && attention_tc5_supported(p)) return launch_attention_tc5(p, (cudaStream_t)stream);
-    ANYSD_REQUIRE(p->lse == nullptr, ANYSD_EUNSUPPORTED, "attention: the log-sum-exp output needs the tcgen05 kernel");
+    const bool want_wg = !force || !strcmp(force, "wgmma");
+    if (want_wg && attention_wg_supported(p)) return launch_attention_wg(p, (cudaStream_t)stream);
+    ANYSD_REQUIRE(p->lse == nullptr, ANYSD_EUNSUPPORTED, "attention: the log-sum-exp output needs the wgmma kernel");
     ANYSD_REQUIRE(!p->aux_cols, ANYSD_EUNSUPPORTED,
-                  "attention: aux_cols needs the tcgen05 kernel (d %% 16 == 8, head_stride >= d + 8, stacked batches)");
+                  "attention: aux_cols needs the wgmma kernel (d %% 16 == 8, head_stride >= d + 8, stacked batches)");
     return launch_attention_mma(p, (cudaStream_t)stream);
 }

@@ -63,8 +63,8 @@ __global__ void silu_bwd_f32_kernel(const float* __restrict__ x, const float* __
 // One thread-block CLUSTER per (image, span of `gpc` whole groups that is also a whole number of 16-byte channel vectors); the
 // cluster's CS CTAs split the HW rows, each with VC = gpc*cpg/8 vector columns x RL row lanes.  Three passes over the slab
 // (statistics; the two sums; dx), the slab stays in L2.  Per-channel partials are folded over the row lanes in smem, then per
-// group, then over the cluster through distributed shared memory in rank order (deterministic).  [measured, round 2] one CTA
-// per slab left the 64x64 level at 128 CTAs with one 16-byte load in flight per thread (118-204 us per launch, ~1 TB/s).
+// group, then over the cluster through distributed shared memory in rank order (deterministic).  One CTA per slab would leave
+// the 64x64 level at 128 CTAs with one 16-byte load in flight per thread.
 constexpr int GNB_THREADS = 256;
 __global__ void __launch_bounds__(GNB_THREADS) gn_bwd_kernel(const __half* __restrict__ x1, int C1, const __half* __restrict__ x2, int C2,
                                                              const float* __restrict__ gamma, const float* __restrict__ beta,
@@ -670,8 +670,8 @@ int anysd_groupnorm_bwd_nhwc_f16(const void* x1, int C1, const void* x2, int C2,
     }
     // CTAs per slab (cluster along x): enough rows per CTA to keep the RL row lanes busy
     static const char* cs_env = getenv("ANYSD_GNBWD_CLUSTER");
-    // [measured, B = 16] 64x64x320: 198 -> 131 us with 8 CTAs per slab; 32x32x640 and below get SLOWER (two cluster barriers per
-    // fold cost more than the parallelism buys): clusters only for the large maps
+    // clusters only for the large maps: on the small ones the two cluster barriers per fold cost more than the parallelism buys
+    // (chosen on the project's earlier GPU, not re-measured on the H100; ANYSD_GNBWD_CLUSTER overrides)
     int CS = HW >= 2048 ? 8 : 1;
     if (cs_env) CS = atoi(cs_env) >= 1 ? atoi(cs_env) : 1;
     cudaLaunchConfig_t cfg = {};

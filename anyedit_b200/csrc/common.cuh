@@ -1,4 +1,4 @@
-// Shared device/host helpers for the anysd_b200 kernels (sm_100a only).
+// Shared device/host helpers for the anysd_b200 kernels (sm_90a only).
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>

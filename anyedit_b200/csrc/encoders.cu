@@ -1,8 +1,8 @@
 // Condition-encoder helpers (SURVEY.md 8f rank 2): everything else of the CLIP towers / Resampler runs on the UNet's kernels
-// (LayerNorm, tcgen05 contractions with fused bias / GELU / QuickGELU / residual, tcgen05 attention).
+// (LayerNorm, wgmma contractions with fused bias / GELU / QuickGELU / residual, wgmma attention).
 //   embed_tokens        CLIPTextEmbeddings (transformers modeling_clip.py): token_embedding[ids] + position_embedding[pos]
 //   attention_small     softmax(q k^T scale [+ causal mask]) v for short sequences: the CLIP text tower's causal 77-token
-//                       self-attention (the tcgen05 attention kernel has no mask path; 77 x 77 x 64 per head is latency-sized)
+//                       self-attention (the wgmma attention kernel has no mask path; 77 x 77 x 64 per head is latency-sized)
 #include "common.cuh"
 
 namespace anysd {

@@ -1,6 +1,6 @@
 // First-stage (autoencoder) helpers, SURVEY.md 8f rank 1 -- everything else of the VAE runs on the UNet's kernels.
 //   softmax_rows   the single-head d = C attention of AttnBlock (ldm/modules/diffusionmodules/model.py:176-203) at C = 512 is
-//                  wider than the tcgen05 attention tile (TMEM holds S + O for d <= 160): it runs as two contractions around a
+//                  wider than the wgmma attention kernel takes (O in registers for d <= 160): it runs as two contractions around a
 //                  row softmax -- S = q k^T (fp32) -> P = softmax(S * C^-0.5) (fp16) -> O = P v.
 //   gaussian       DiagonalGaussianDistribution (ldm/modules/distributions/distributions.py:24-62): clamp, std, sample.
 #include "common.cuh"

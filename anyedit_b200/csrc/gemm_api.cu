@@ -6,12 +6,10 @@
 
 namespace anysd {
 int launch_gemm_mma(const anysd_gemm_params* q, cudaStream_t st);
-int launch_gemm_tc5(const anysd_gemm_params* q, cudaStream_t st);
-bool tc5_supported(const anysd_gemm_params* q);
-int launch_gemm_tc5p(const anysd_gemm_params* q, cudaStream_t st);
-bool tc5p_supported(const anysd_gemm_params* q);
-int tc5p_stats_slabs(const anysd_gemm_params* q);
-size_t tc5p_splitk_bytes(const anysd_gemm_params* q);
+int launch_gemm_wg(const anysd_gemm_params* q, cudaStream_t st);
+bool wg_supported(const anysd_gemm_params* q);
+int wg_stats_slabs(const anysd_gemm_params* q);
+size_t wg_splitk_bytes(const anysd_gemm_params* q);
 }
 
 using namespace anysd;
@@ -51,36 +49,33 @@ extern "C" int anysd_gemm_f16(const anysd_gemm_params* p, anysd_stream_t stream)
         ANYSD_REQUIRE(p->lda % 8 == 0 && p->lda >= p->K, ANYSD_EINVAL, "gemm: lda=%d must be a multiple of 8 and >= K",
                       p->lda);
     }
-    // Kernel selection.  The persistent tcgen05/TMA kernel (gemm_tc5p.cu) takes every fp16-output contraction
-    // whose layout constraints hold: all nn.Linear / 1x1 convs and every 3x3 conv with Cin % 64 == 0 (stride 1|2,
-    // upsample through the workspace).  The one-tile-per-CTA tcgen05 kernel (gemm_tc5.cu) takes the fp32-output
-    // ones (time-embedding path).  mma.sync covers what is left: the Cin = 8 input conv and the N = 4 output conv.
-    // ANYSD_GEMM=mma|tc5|tc5p is a test/debug switch used to cross-check the kernels against each other.
+    // Kernel selection.  The persistent wgmma/TMA kernel (gemm_wgmma.cu) takes every contraction whose layout constraints
+    // hold: all nn.Linear / 1x1 convs and every 3x3 conv with Cin % 64 == 0 (stride 1|2, upsample through the workspace),
+    // fp16 or fp32 output.  mma.sync covers what is left (Cin % 64 != 0 convs, N % 8 != 0).
+    // ANYSD_GEMM=mma is a test/debug switch used to cross-check the two kernels against each other.
     static const char* force = getenv("ANYSD_GEMM");
-    const bool allow_p = !force || !strcmp(force, "tc5p");
-    const bool allow_1 = !force || !strcmp(force, "tc5");
-    if (allow_p && tc5p_supported(p)) return launch_gemm_tc5p(p, (cudaStream_t)stream);
+    const bool allow_wg = !force || !strcmp(force, "wgmma");
+    if (allow_wg && wg_supported(p)) return launch_gemm_wg(p, (cudaStream_t)stream);
     ANYSD_REQUIRE(p->row_stats == nullptr && p->ln_stats == nullptr, ANYSD_EUNSUPPORTED,
-                  "gemm: LayerNorm fold / row statistics need the persistent tcgen05 path");
-    ANYSD_REQUIRE(p->stats == nullptr, ANYSD_EUNSUPPORTED, "gemm: output statistics need the persistent tcgen05 path");
+                  "gemm: LayerNorm fold / row statistics need the persistent wgmma path");
+    ANYSD_REQUIRE(p->stats == nullptr, ANYSD_EUNSUPPORTED, "gemm: output statistics need the persistent wgmma path");
     ANYSD_REQUIRE(!(p->conv && p->conv_pad), ANYSD_EUNSUPPORTED,
-                  "conv3x3 with right/bottom padding needs the persistent tcgen05 path (fp16 output, Cin %% 64 == 0)");
-    if ((allow_1 || (force && !strcmp(force, "tc5p"))) && tc5_supported(p)) return launch_gemm_tc5(p, (cudaStream_t)stream);
+                  "conv3x3 with right/bottom padding needs the persistent wgmma path (Cin %% 64 == 0)");
     return launch_gemm_mma(p, (cudaStream_t)stream);
 }
 
 extern "C" int anysd_gemm_stats_slabs(const anysd_gemm_params* p) {
     if (p == nullptr || !p->A || !p->W || !p->out) return 0;
     static const char* force = getenv("ANYSD_GEMM");
-    if (force && strcmp(force, "tc5p")) return 0;
+    if (force && strcmp(force, "wgmma")) return 0;
     if (p->conv && (p->Cin <= 0 || p->K != 9 * p->Cin)) return 0;
-    return tc5p_supported(p) ? tc5p_stats_slabs(p) : 0;
+    return wg_supported(p) ? wg_stats_slabs(p) : 0;
 }
 
 extern "C" size_t anysd_gemm_splitk_workspace_bytes(const anysd_gemm_params* p) {
     if (p == nullptr || !p->A || !p->W || !p->out) return 0;
     static const char* force = getenv("ANYSD_GEMM");
-    if (force && strcmp(force, "tc5p")) return 0;
+    if (force && strcmp(force, "wgmma")) return 0;
     if (p->conv && (p->Cin <= 0 || p->K != 9 * p->Cin)) return 0;
-    return tc5p_supported(p) ? tc5p_splitk_bytes(p) : 0;
+    return wg_supported(p) ? wg_splitk_bytes(p) : 0;
 }

@@ -4,8 +4,8 @@
 // upsample folded into the gather coordinates, zero-fill halo through cp.async src-size 0).
 // Epilogue (fp32): + bias[n] + rowadd[m / rows_per_batch, n] -> SiLU | GEGLU -> + residual -> fp16|fp32.
 //
-// This is the correctness baseline the tcgen05 kernels (gemm_tc5.cu) are validated against;
-// the dispatch in anysd_gemm_f16 prefers tcgen05 wherever its shape constraints hold.
+// This is the correctness baseline the wgmma kernel (gemm_wgmma.cu) is validated against;
+// the dispatch in anysd_gemm_f16 prefers wgmma wherever its shape constraints hold.
 #include "common.cuh"
 
 namespace anysd {

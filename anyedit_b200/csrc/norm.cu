@@ -382,11 +382,9 @@ __global__ void __launch_bounds__(512, 2) gn_fused_kernel(const GnFusedArgs a) {
 // two-pass sums (mean, then centred squares: no E[x^2] - mean^2 cancellation) folded in a fixed order: thread -> 8 row lanes ->
 // group (one warp, lane-strided + shuffle tree).  The decomposition is a function of (C, HW, G) only, so every output bit is
 // independent of the batch.  Against the cooperative statistics + apply kernel: no second read of x, no grid barrier.
-// [measured, B200, batch 16, tests/diag_gn.py, profiles/r2_diag_gn_resident.txt] 16x16x1280: 14.9 vs 18.9 us; 8x8x1280: 10.9 vs
-// 14.3; 16x16x2560: 19.5 vs 35.4; 8x8x2560: 13.8 vs 14.9.  A cluster version of the same kernel (up to 16 CTAs per span splitting
-// the rows, partials exchanged through distributed shared memory) was built for the large maps and was SLOWER than the
-// epilogue-statistics path: 64x64x320 46.5 us (vs 31), 64x64x960 202 us (vs 69), 32x32x640 23.2 (vs 21.3) -- two cluster
-// barriers + the remote reads are ~5 us of latency per CTA that two resident CTAs per SM cannot hide -- so it is not kept.
+// A cluster version of the same kernel (up to 16 CTAs per span splitting the rows, partials exchanged through distributed shared
+// memory) was built for the large maps and was slower than the epilogue-statistics path -- two cluster barriers + the remote
+// reads are latency that two resident CTAs per SM cannot hide -- so it is not kept.
 struct GnResArgs {
     const uint4* x1; const uint4* x2; uint4* y;
     const float* gamma; const float* beta;
@@ -548,7 +546,7 @@ static int launch_gn_res(const GnResPlan& pl, const void* x1, int C1, const void
 // ---- LayerNorm: LPR lanes per token row (8 / 16 / 32), VPL 16-byte vectors per lane held in registers ---------
 // C = 320 / 640 / 1280 map to LPR = 8 / 16 / 32 with exactly 5 vectors per lane: a warp then normalises
 // 4 / 2 / 1 rows at once with 5 independent 16-byte loads in flight per lane (the one-warp-per-row version left
-// 24 of 32 lanes with a single load at C = 320 and ran at 1.6 TB/s).  Two-pass exact variance from registers.
+// 24 of 32 lanes with a single load at C = 320).  Two-pass exact variance from registers.
 template <int LPR, int VPL>
 __global__ void layernorm_kernel(const uint4* __restrict__ x, const float* __restrict__ gamma,
                                  const float* __restrict__ beta, uint4* __restrict__ y, long long M, int CV, float eps) {

@@ -1,4 +1,4 @@
-"""Condition encoders on the B200 kernels (SURVEY.md 8f rank 2): what produces ``c_crossattn`` and the visual tokens right
+"""Condition encoders on the H100 kernels (SURVEY.md 8f rank 2): what produces ``c_crossattn`` and the visual tokens right
 before the denoising loop.
 
   ``FrozenCLIPEmbedder``            ldm/modules/encoders/modules.py:107-150 -- the CLIP text tower the ``ldm`` stack conditions on
@@ -14,8 +14,8 @@ before the denoising loop.
 
 The arithmetic of the two CLIP towers lives in a third-party dependency of the reference (``transformers``, unpinned in
 requirements.txt; 5.5 is what this image has): the golden vectors are generated from that library's own modules with seeded
-weights (tests/golden/make_golden_encoders.py).  Execution: LayerNorm kernel, tcgen05 contractions with bias / QuickGELU /
-GELU / residual fused in the epilogue, the tcgen05 attention kernel for the vision tower and the Resampler, the short-sequence
+weights (tests/golden/make_golden_encoders.py).  Execution: LayerNorm kernel, wgmma contractions with bias / QuickGELU /
+GELU / residual fused in the epilogue, the wgmma attention kernel for the vision tower and the Resampler, the short-sequence
 causal attention kernel for the 77 text tokens.  Tokenisation (vocabulary files) is outside the path: the text tower takes
 token ids (or a caller-supplied tokenizer).  No eager-PyTorch math, no CPU fallback.
 """

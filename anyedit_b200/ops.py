@@ -1,7 +1,7 @@
 """Torch-tensor wrappers over the C ABI (include/anysd_b200.h).
 
 PyTorch is plumbing here: device memory, the current CUDA stream, nothing else.  Every function
-launches hand-written sm_100a kernels from ``libanysd_b200.so`` on ``torch.cuda.current_stream()``
+launches hand-written sm_90a kernels from ``libanysd_b200.so`` on ``torch.cuda.current_stream()``
 and raises on failure.  Tensors are NHWC / token-major fp16 unless stated.
 """
 import os
@@ -201,10 +201,10 @@ class GnStats:
 def _want_stats(p, images, dev, reuse=None):
     """Allocate the statistics buffer when the launch can fill it (anysd_gemm_stats_slabs); returns GnStats or None.
     ``reuse``: a GnStats of the same geometry whose buffer is refilled (persistent outputs read by a captured graph)."""
-    # [measured, tests/diag_gn.py, batch 16] finalize + streaming apply vs the one-launch statistics + apply kernel:
-    # 31 vs 42 us (64x64 map, 320 ch), 21 vs 29 us (32x32, 640 ch), 69 vs 103 us (64x64, 960 ch) -- but 23 vs 19 us at 16x16
-    # and 15 vs 14 us at 8x8, where two launches cost more than the statistics pass they replace: maps of >= 1024 pixels only
-    # (below that the register-resident kernel -- anysd_groupnorm_resident -- reads x once and needs no statistics)
+    # finalize + streaming apply pays against the one-launch statistics + apply kernel on the large maps only; on the small ones
+    # two launches cost more than the statistics pass they replace: maps of >= 1024 pixels only (below that the
+    # register-resident kernel -- anysd_groupnorm_resident -- reads x once and needs no statistics).  The threshold was chosen
+    # with tests/diag_gn.py on the project's earlier GPU and has not been re-measured on the H100.
     if not _GN_EPILOGUE or p.rows_per_batch < GN_EPILOGUE_MIN_ROWS:
         return None
     S = _lib.load().anysd_gemm_stats_slabs(C.byref(p))
@@ -317,7 +317,7 @@ def conv3x3(x, W, out, bias=None, rowadd=None, residual=None, stride=1, upsample
     p.conv_pad = int(bool(pad_rb))
     p.Nimg, p.H, p.Wd, p.Cin = Nimg, H, Wd, Cin
     p.stride, p.upsample = stride, upsample
-    if upsample:   # scratch for the materialised nearest-x2 input of the tcgen05 path
+    if upsample:   # scratch for the materialised nearest-x2 input of the wgmma path
         ws = torch.empty(Nimg * Hl * Wl * Cin, dtype=torch.float16, device=x.device)
         p.workspace, p.workspace_bytes = ws.data_ptr(), ws.numel() * 2
     # algorithmic FLOPs (trace only): zero-padded channels do not count
@@ -529,7 +529,7 @@ def attention_bwd(q, k, v, d_out, dq, dk, dv, B, heads, n_q, n_kv, d, ld_q, ld_k
     ws = torch.empty(nbytes // 4, dtype=torch.float32, device=q.device)
     p.workspace, p.workspace_bytes = ws.data_ptr(), nbytes
     dpad = None
-    if lse is not None and out is not None:        # the tcgen05 kernels (shape permitting; the library decides)
+    if lse is not None and out is not None:        # the wgmma kernels (shape permitting; the library decides)
         assert lse.dtype == torch.float32 and lse.is_contiguous() and lse.numel() == B * heads * n_q
         hs = head_stride if head_stride > 0 else d
         dpad = torch.empty(B * n_q * heads * hs, dtype=torch.float16, device=q.device)

@@ -1,4 +1,4 @@
-"""Training step of the AnySD adapters (SURVEY.md a24; reference train.py:629-710) on the B200 kernels.
+"""Training step of the AnySD adapters (SURVEY.md a24; reference train.py:629-710) on the H100 kernels.
 
 The reference runs ``loss = mse(MoE(cat(q_sample(z, eps, t), z_orig), t, text, ref_embeds, edit_code), eps)``,
 ``loss.backward()`` through a FROZEN UNet (train.py:415) and AdamW over the adapter tensors (:486-492).  Here the
@@ -43,10 +43,8 @@ def conditioning_dropout(text, null_text, image_latent, random_p, prob):
 
 # Gradient all-reduce schedule.  ANYSD_TRAIN_ALLREDUCE=end (default): ONE all-reduce of the whole flat gradient buffer after the
 # backward; =overlap: each layer's region is all-reduced as soon as it is final, under the rest of the backward (DDP bucket
-# semantics).  [measured, 2 x B200, batch 16 per GPU, profiles/r2_train_allreduce.md] 74.8 ms per step on one GPU; overlap 80.3 ms,
-# overlap with NCCL_MAX_CTAS=4 76.9 ms, end 76.9 ms: NCCL's CTAs take SMs the persistent one-CTA-per-SM contraction kernels count
-# on (a 148-CTA grid with a few SMs occupied runs its last CTAs as a second wave), which costs more than the 2.2 ms the 0.85 GB
-# collective takes at full speed on its own.
+# semantics).  The default keeps NCCL's CTAs off the SMs while the persistent one-CTA-per-SM contraction kernels run (a full
+# grid with a few SMs occupied runs its last CTAs as a second wave).
 _AR_OVERLAP = os.environ.get("ANYSD_TRAIN_ALLREDUCE", "end") == "overlap"
 
 
@@ -522,7 +520,7 @@ class AdapterTrainer:
         if ctx is None:
             qkv = torch.empty(N * n_q, 3 * Cp, dtype=torch.float16, device=dev)
             ops.gemm(xq, ad["qkv_w"], qkv, bias=ad["qkv_b"])
-            # the long small-head self-attention keeps its log-sum-exp: the backward then runs on the tcgen05 kernels
+            # the long small-head self-attention keeps its log-sum-exp: the backward then runs on the wgmma kernels
             d_ext = (ad["d"] + 15) // 16 * 16
             lse = torch.empty(N, ad["heads"], n_q, dtype=torch.float32, device=dev) if (d_ext <= 64 and hs == d_ext and n_q % 128 == 0) else None
             ops.attention(qkv, qkv[:, Cp:], qkv[:, 2 * Cp:], a, N, ad["heads"], n_q, n_q, ad["d"], 3 * Cp, 3 * Cp, 3 * Cp, C,

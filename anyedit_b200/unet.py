@@ -1,4 +1,4 @@
-"""B200-native ``UNetModel`` -- drop-in for ``ldm.modules.diffusionmodules.openaimodel.UNetModel``.
+"""H100-native ``UNetModel`` -- drop-in for ``ldm.modules.diffusionmodules.openaimodel.UNetModel``.
 
 Same constructor kwargs (openaimodel.py:442-472), same ``state_dict`` keys and shapes
 (SURVEY.md 8b: 686 tensors for the SD-1.5 geometry) and the same call
@@ -6,7 +6,7 @@ Same constructor kwargs (openaimodel.py:442-472), same ``state_dict`` keys and s
 strings, checkpoints and ``DDIMSampler`` keep working.  What differs is the execution: the
 parameters are repacked once into kernel layouts (fp16, conv weights as [Cout, (ky,kx,ci)],
 fused QKV / KV, interleaved GEGLU, all 22 ``emb_layers`` stacked into one matrix) and the
-forward is a fixed sequence of hand-written sm_100a kernels on NHWC fp16 activations,
+forward is a fixed sequence of hand-written sm_90a kernels on NHWC fp16 activations,
 launched through the C ABI in ``include/anysd_b200.h``.  No eager-PyTorch math, no fallback.
 
 Supported configuration = what the AnySD / SD-1.5 / anydoor.yaml geometries use:
@@ -153,10 +153,9 @@ class _Embedding(nn.Module):
 # ---- packed (kernel-layout) weights -------------------------------------------------------------
 
 # LayerNorm folded into the contractions either side of it (row moments from the producer's epilogue, gamma / beta folded into the
-# consumer's weights: anysd_gemm_params::row_stats / ln_stats).  OFF by default: [measured, B200, tests/diag_lnfold.py,
-# profiles/r2_lnfold_*.txt] the consumers are epilogue-bound contractions (K = 320 .. 1280) and the two extra FMAs + the
-# column-sum operand per accumulator cost them more (GEGLU 65536 x 2560 x 320: 140 -> 167 us even with every parameter
-# staged in shared memory) than the 21 us layernorm launch they replace; ANYSD_LN_FOLD=1 switches it on.
+# consumer's weights: anysd_gemm_params::row_stats / ln_stats).  OFF by default: the consumers are
+# epilogue-bound contractions (K = 320 .. 1280) and the two extra FMAs + the column-sum operand per accumulator can cost them
+# more than the layernorm launch they replace; ANYSD_LN_FOLD=1 switches it on.
 _LN_FOLD = os.environ.get("ANYSD_LN_FOLD", "0")[:1] == "1"
 
 
@@ -169,7 +168,7 @@ def _f(t, dev):
 
 
 def head_stride_for(d):
-    """Head stride of packed q/k/v projections: d, or ceil16(d) when d is not a multiple of 16 -- the tcgen05
+    """Head stride of packed q/k/v projections: d, or ceil16(d) when d is not a multiple of 16 -- the wgmma
     attention kernel contracts over ceil16(d) columns and needs the extra ones to be exact zeros (d = 40 -> 48)."""
     return d if d % 16 == 0 else (d + 15) // 16 * 16
 
@@ -365,8 +364,8 @@ class UNetModel(nn.Module):
         P["te2_w"], P["te2_b"] = _h(te[2].weight, dev), _f(te[2].bias, dev)
         if self.num_classes is not None:
             P["label"] = _f(self.label_emb.weight, dev)
-        # input channels padded to 64 (zeros) so that the input conv runs on the tcgen05 implicit-GEMM kernel
-        # (64-channel k-blocks); the extra MACs are on zero weights and cost ~25 us per forward
+        # input channels padded to 64 (zeros) so that the input conv runs on the wgmma implicit-GEMM kernel
+        # (64-channel k-blocks); the extra MACs are on zero weights
         self._cin_pad = (self.in_channels + 63) // 64 * 64
         P["in_w"] = _pack_conv3(self.input_blocks[0][0].weight, dev, self._cin_pad)
         P["in_b"] = _f(self.input_blocks[0][0].bias, dev)
@@ -456,7 +455,7 @@ class UNetModel(nn.Module):
             self._pack, self._pack_key = P, key
             return P
         P["out_gn_w"], P["out_gn_b"] = _f(self.out[0].weight, dev), _f(self.out[0].bias, dev)
-        # output conv: rows padded to a multiple of 8 (zero filters) -> tcgen05 kernel with fp32 output
+        # output conv: rows padded to a multiple of 8 (zero filters) -> wgmma kernel with fp32 output
         self._cout_pad = (self.out_channels + 7) // 8 * 8
         ow = _pack_conv3(self.out[2].weight, dev)
         ob = _f(self.out[2].bias, dev)

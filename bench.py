@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- edited images/sec at 512x512 / 50-step DDIM / CFG (BASELINE.json metric).
 
-    python bench.py --gpus N --steps K --warmup W [--impl reference]
+    python bench.py --gpus N --steps K --warmup W [--impl reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 A "step" = one complete CFG DDIM sampling run (``DDIMSampler.sample``: 50 UNet evaluations on the
@@ -9,6 +9,10 @@ CFG-doubled batch + 50 fused updates) over one batch of synthetic edit requests.
 N = BASELINE configs[1] per GPU (512x512 "replace" edit -> 64x64 latent, 50 DDIM steps, CFG 7.5,
 batch 8, SD-1.5/IP2P UNet geometry with 8 input channels and 77x768 text context); N GPUs run N
 such batches (weak scaling), no collective inside the loop.
+
+--dump-outputs DIR writes what the timed path returned in its last timed step -- the sampled latents of the batch,
+DIR/samples.npy, float32 [batch, 4, latent, latent] -- so that two builds can be compared output for output (the inputs
+and the random-init weights are seeded: identical from run to run).
 
 Prints ONE JSON line (rank 0).  ``value`` is device-resident throughput, ``e2e`` the same metric
 through the public API with pinned-host inputs/outputs inside the timed region.  The same line carries
@@ -59,6 +63,8 @@ def parse():
     ap.add_argument("--extra", default="C2,C3,C4,dpm20,pipeline", help="comma list of extra legs to run")
     ap.add_argument("--c2-total", type=int, default=64, help="configs[2]: requests summed over all GPUs")
     ap.add_argument("--c2-chunk", type=int, default=16, help="configs[2]: requests per sampling call on one GPU")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the headline leg's last timed outputs as DIR/<name>.npy (float32)")
     return ap.parse_args()
 
 
@@ -223,7 +229,7 @@ def workload_config(args, world):
                         f"(SD-1.5/IP2P UNet geometry: in=8, 320ch, mult 1-2-4-4, 8 heads, ctx 77x768)",
             "global_batch": args.batch * world, "latent": args.latent, "ddim_steps": args.ddim_steps,
             "guidance_scale": args.scale, "parallelism": f"dp{world} (requests sharded, no in-loop collective)",
-            "l2_policy": "working set > L2 every step (1.72 GB fp16 weights + >1 GB activations vs 126 MB L2)"}
+            "l2_policy": "working set > L2 every step (1.72 GB fp16 weights + >1 GB activations vs 50 MB L2)"}
 
 
 def synth_requests(B, h, seed, n_vis=0, vis_zero=False, first_index=0):
@@ -294,9 +300,10 @@ def main():
         D.barrier()
         return D.max_over_ranks(e0.elapsed_time(e1) / 1e3, dev)
 
-    def sampling_leg(sampler_obj, hosts, S, h, scale, warmup, steps, method="ddim"):
+    def sampling_leg(sampler_obj, hosts, S, h, scale, warmup, steps, method="ddim", keep=None):
         """Times `steps` passes over the list of request chunks `hosts` (each one sampler call), resident and e2e.
-        Returns (t_resident, t_e2e, kernel launches per resident pass, h2d bytes, d2h bytes)."""
+        Returns (t_resident, t_e2e, kernel launches per resident pass, h2d bytes, d2h bytes); `keep` (a dict) receives the
+        outputs of the last timed resident pass under "out" (one tensor per chunk)."""
         outs = [torch.empty(hh["x_T"].shape).pin_memory() for hh in hosts]
 
         def run(devt):
@@ -308,8 +315,9 @@ def main():
         devs = [{k: v.to(dev) for k, v in hh.items()} for hh in hosts]
 
         def resident():
-            for d_ in devs:
-                run(d_)
+            outs_dev = [run(d_) for d_ in devs]
+            if keep is not None:
+                keep["out"] = outs_dev
 
         def e2e():
             for hh, oh in zip(hosts, outs):
@@ -340,7 +348,12 @@ def main():
         clocks.start()
     if os.environ.get("ANYSD_NCU"):      # ncu --profile-from-start off: launch list of the timed region only
         torch.cuda.cudart().cudaProfilerStart()
-    t_res, t_e2e, launches, h2d, d2h = sampling_leg(sampler, [host], S, h, args.scale, 0, args.steps)
+    kept = {}
+    t_res, t_e2e, launches, h2d, d2h = sampling_leg(sampler, [host], S, h, args.scale, 0, args.steps, keep=kept)
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "samples.npy"), kept["out"][0].detach().float().cpu().numpy())
     launches *= args.steps                # the headline reports the launches of the whole timed region
     if os.environ.get("ANYSD_NCU"):
         torch.cuda.cudart().cudaProfilerStop()
@@ -354,8 +367,8 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak = peaks.get("bf16_tflops_sustained", 1400.0)
-    peak_src = "MEASURED_PEAKS.json bf16_tflops_sustained (of measured)" if peaks else "fallback 1400 (B200_PROFILING.md)"
+    peak = peaks.get("bf16_tflops_sustained", 989.0)
+    peak_src = "MEASURED_PEAKS.json bf16_tflops_sustained (of measured)" if peaks else "H100 SXM data sheet, dense FP16 (989 TFLOP/s at 700 W)"
 
     # ---- parity of the timed path: eps of request 0 in the LAST graph replay vs the CPU reference ----
     parity = None
@@ -387,14 +400,8 @@ def main():
         gemm_f = agg.get("gemm", [0, 0, 0])[0] + agg.get("conv3x3", [0, 0, 0])[0]
         gemm_t = agg.get("gemm", [0, 1e-9, 0])[1] + agg.get("conv3x3", [0, 0, 0])[1]
         ach = gemm_f / gemm_t / 1e12
-        traffic = None
-        try:
-            traffic = json.load(open(os.path.join(ROOT, "profiles", "dominant_kernel_traffic.json"))).get("bytes_per_launch")
-        except Exception:
-            pass
         roof = {"bound": "tensor", "kernel": "implicit-GEMM conv3x3 + linear contraction (anysd_gemm_f16)",
                 "achieved": ach, "peak": peak, "unit": "TFLOP/s", "frac": ach / peak, "peak_source": peak_src,
-                "traffic": traffic,
                 "per_kind": {k: {"tflops": (v[0] / v[1] / 1e12) if v[0] else None, "ms": v[1] * 1e3, "launches": v[2], "gflop": v[0] / 1e9}
                              for k, v in agg.items()},
                 "whole_step_tflops": 2 * S * F_UNET[h] * B * world * args.steps / t_res / 1e12 if h in F_UNET else None}

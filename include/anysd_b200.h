@@ -1,4 +1,4 @@
-/* anysd_b200 -- C ABI of the B200-native AnySD denoising hot path.
+/* anysd_b200 -- C ABI of the H100-native AnySD denoising hot path (the name is historical).
  *
  * The reference (DCDmllm/AnyEdit) has no FFI boundary on this path: its hot path is eager
  * PyTorch modules (SURVEY.md 8b).  This header is therefore the *new* boundary a maintainer
@@ -155,7 +155,7 @@ typedef struct {
 } anysd_gemm_params;
 int anysd_gemm_f16(const anysd_gemm_params* p, anysd_stream_t stream);
 /* Slabs per image of the statistics layout for this contraction, or 0 when the shape cannot produce them (rows of one
- * image not a multiple of 32, conv patches not tiling the image exactly, GEGLU / fp32 output, non-tcgen05 shape). */
+ * image not a multiple of 32, conv patches not tiling the image exactly, GEGLU / fp32 output, a shape the wgmma kernel does not take). */
 int anysd_gemm_stats_slabs(const anysd_gemm_params* p);
 /* Bytes of `splitk_workspace` with which this contraction runs split-K (0: the schedule does not split it).  Whether a layer is
  * split depends on its per-image geometry only (<= 128 output rows per image and a long K), never on the batch; the partial
@@ -178,17 +178,16 @@ typedef struct {
     const float* gate;      /* [B] stride gate_stride, or NULL */
     int gate_stride;
     int accumulate;
-    int head_stride;        /* elements between consecutive heads inside a q/k/v row; 0 = d.  The tcgen05 kernel
+    int head_stride;        /* elements between consecutive heads inside a q/k/v row; 0 = d.  The wgmma kernel
                                needs head_stride >= ceil16(d) with zero padding columns when d % 16 != 0 */
-    int aux_cols;           /* 1 = "operands carry the softmax bookkeeping" (tcgen05 kernel only; needs d % 16 == 8,
+    int aux_cols;           /* 1 = "operands carry the softmax bookkeeping" (wgmma kernel only; needs d % 16 == 8,
                                head_stride >= d + 8, EUNSUPPORTED otherwise).  Contract, per head:
                                  q: columns [0,d) hold q * scale * log2(e) (the caller folds both into Wq; `scale` is
                                     ignored), columns d.. are zero;
                                  k: columns d and d+1 hold 1.0;    v: column d holds 1.0;   other padding zero.
-                               The kernel writes its running reference into q's padding inside shared memory, so the
-                               scores leave the tensor core already shifted (exp2 only) and the softmax denominator is
-                               column d of P.V.  Same result as aux_cols = 0 up to fp32 rounding. */
-    float* lse;             /* optional OUTPUT (tcgen05 kernels only, gate == NULL): fp32 [B, heads, n_q], the base-2 log-sum-exp of
+                               The padding columns meet zeros in Q K^T, so the kernel runs these operands with a unit
+                               scale.  Same result as aux_cols = 0 up to fp32 rounding. */
+    float* lse;             /* optional OUTPUT (wgmma kernel only, gate == NULL): fp32 [B, heads, n_q], the base-2 log-sum-exp of
                                every score row, lse2_i = log2 sum_j 2^(scale log2(e) q_i.k_j) -- what anysd_attention_bwd_f16 needs
                                to recompute the probabilities without its own pass over K (train.py:694-709 backward). */
 } anysd_attn_params;
@@ -246,7 +245,7 @@ int anysd_gaussian_posterior_f32(const float* moments, const float* noise, float
 int anysd_embed_tokens_f16(const long long* ids, const void* tok_table, const void* pos_table, void* out, int B, int n, int D,
                            int vocab, anysd_stream_t stream);
 /* softmax(q k^T scale [+ causal mask]) v per (batch, head) for SHORT sequences (n_kv <= 256): the causal 77-token
- * self-attention of the CLIP text tower (the tcgen05 attention has no mask path).  Row-major fp16 q [B*n_q, ld_q] with head h
+ * self-attention of the CLIP text tower (the wgmma attention has no mask path).  Row-major fp16 q [B*n_q, ld_q] with head h
  * at columns [h d, (h+1) d), same for k, v ([B*n_kv, ld_k|ld_v]) and out; causal != 0: key j masked for query i when j > i. */
 int anysd_attention_small_f16(const void* q, const void* k, const void* v, void* out, int B, int heads, int n_q, int n_kv, int d,
                               int ld_q, int ld_k, int ld_v, int ld_o, float scale, int causal, anysd_stream_t stream);
@@ -312,8 +311,8 @@ typedef struct {
                                sweep over K/V.  NULL: recomputed. */
     long long o_batch_stride; int ld_o;
     const float* lse;       /* optional: the forward's anysd_attn_params::lse ([B, heads, n_q], base 2).  With `lse`, `out` and */
-    void* dout_padded;      /* `dout_padded` (scratch, fp16 [B, n_q, heads * head_stride]) the backward runs on the tcgen05 kernels
-                               (attention_bwd_tc5.cu) when the shape allows: ceil16(d) <= 64 == head_stride, n_q and n_kv multiples
+    void* dout_padded;      /* `dout_padded` (scratch, fp16 [B, n_q, heads * head_stride]) the backward runs on the wgmma kernels
+                               (attention_wgmma.cu) when the shape allows: ceil16(d) <= 64 == head_stride, n_q and n_kv multiples
                                of 128, stacked batches, no gate; otherwise both are ignored. */
 } anysd_attn_bwd_params;
 size_t anysd_attention_bwd_workspace_bytes(int B, int heads, int n_q);

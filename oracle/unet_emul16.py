@@ -15,10 +15,10 @@ Rounding points (file:line of the kernel that rounds):
   weights                      -> fp16 once at pack time (anyedit_b200/unet.py _h / _pack_conv3); for heads with
                                   d % 16 == 8 the query weight is multiplied by d^-0.5 * log2(e) BEFORE rounding (unet.py:381-386)
   every GEMM / conv output     -> fp16 after bias + time-embedding row + activation + residual in fp32
-                                  (csrc/gemm_tc5p.cu epilogue); the time-embedding linears and the output conv stay fp32
+                                  (csrc/gemm_wgmma.cu epilogue); the time-embedding linears and the output conv stay fp32
   GroupNorm(+SiLU) / LayerNorm -> fp32 statistics, fp16 output (csrc/norm.cu)
-  attention                    -> fp32 scores, P rounded to fp16 before P.V, output fp16 (csrc/attention_tc5.cu); the
-                                  denominator is the sum of the ROUNDED P when d % 16 == 8 (aux columns), of the unrounded P otherwise
+  attention                    -> fp32 scores, P rounded to fp16 before P.V, output fp16 (csrc/attention_wgmma.cu); the
+                                  denominator is the sum of the unrounded fp32 P (with or without aux columns)
   GEGLU                        -> a * gelu(gate) in fp32, fp16 output
   timestep embedding, silu(emb)-> fp16 (csrc/elementwise.cu)
 Reference structure: the same file:line map as oracle/unet_oracle.py.
@@ -90,7 +90,7 @@ def _attn_core(q, k, v, heads, d, aux):
     s = s - s.amax(-1, keepdim=True)
     p = torch.exp2(s)
     p16 = r16(p)
-    den = (p16 if aux else p).sum(-1, keepdim=True)
+    den = p.sum(-1, keepdim=True)
     o = torch.matmul(p16, vh) / den
     return r16(o.permute(0, 2, 1, 3).reshape(B, n, heads * d))
 

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Diagnostic (not a pytest file): attention kernel timing on the UNet's shapes. ANYSD_ATTN=mma|tc5 selects the kernel."""
+"""Diagnostic (not a pytest file): attention kernel timing on the UNet's shapes. ANYSD_ATTN=mma|wgmma selects the kernel."""
 import os
 import sys
 

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Diagnostic (not a pytest file): the three dominant kernels on their bench shapes, each launched twice, for
-   ncu --set full --clock-control none --import-source on -k regex:"attention_tc5|gemm_tc5p|bwd_d" -o gpurun_out/prof python tests/diag_profile.py"""
+   ncu --set full --clock-control none --import-source on -k regex:"attention_wgmma|gemm_wgmma|bwd_d" -o prof python tests/diag_profile.py"""
 import os
 import sys
 
@@ -41,7 +41,7 @@ bg = rn(2560) * 0.1
 o3 = torch.empty(B * 4096, 1280, dtype=torch.float16, device="cuda")
 for _ in range(2):
     ops.gemm(a, wg, o3, bias=bg, act=2)
-# 4. backward of 1. on the tcgen05 kernels (the forward keeps its log-sum-exp)
+# 4. backward of 1. (the forward keeps its log-sum-exp)
 lse = torch.empty(B, heads, n, dtype=torch.float32, device="cuda")
 ops.attention(qkv, qkv[:, Cp:], qkv[:, 2 * Cp:], out, B, heads, n, n, d, 3 * Cp, 3 * Cp, 3 * Cp, heads * d, head_stride=hs, aux_cols=True, lse=lse)
 d_out = (rn(B * n, heads * d) * 0.1).half()

@@ -27,8 +27,7 @@ def timeit(fn, iters=20):
 def main():
     B = 16
     g = torch.Generator(device="cuda").manual_seed(2)
-    print("ANYSD_GEMM_SPLITK =", os.environ.get("ANYSD_GEMM_SPLITK"), "ANYSD_GEMM_BN =", os.environ.get("ANYSD_GEMM_BN"),
-          "ANYSD_GEMM_CTAS =", os.environ.get("ANYSD_GEMM_CTAS"), flush=True)
+    print("ANYSD_GEMM_SPLITK =", os.environ.get("ANYSD_GEMM_SPLITK"), "ANYSD_GEMM_BN =", os.environ.get("ANYSD_GEMM_BN"), flush=True)
     for (Cin, Cout, H, W, res) in ((1280, 1280, 8, 8, True), (2560, 1280, 8, 8, False), (1280, 1280, 16, 16, True)):
         x = torch.randn(B, H, W, Cin, device="cuda", generator=g).half()
         w = (torch.randn(Cout, 9 * Cin, device="cuda", generator=g) * (9 * Cin) ** -0.5).half()

@@ -25,7 +25,7 @@ def ops():
         pytest.skip("no CUDA device")
     from anyedit_b200 import ops as o
     sms, major, minor = o.device_info()
-    assert major >= 10, f"sm_100a kernels need a Blackwell GPU, got cc {major}.{minor}"
+    assert (major, minor) == (9, 0), f"sm_90a kernels need a Hopper GPU (H100), got cc {major}.{minor}"
     return o
 
 
@@ -336,7 +336,7 @@ def test_errors_are_loud(ops):
                                               (1, 8, 1024, 1024, 40), (1, 3, 130, 513, 24)])
 def test_attention_padded_heads(ops, B, heads, nq, nkv, d):
     """Head stride padded to ceil16(d) with zero columns (the layout anyedit_b200.unet packs when d % 16 != 0,
-    required by the tcgen05 kernel): same result as the unpadded reference."""
+    required by the wgmma kernel): same result as the unpadded reference."""
     from anyedit_b200.unet import head_stride_for
     from oracle import unet_oracle
     hs = head_stride_for(d)
@@ -366,9 +366,8 @@ def test_attention_padded_heads(ops, B, heads, nq, nkv, d):
 def test_attention_aux_cols(ops, B, heads, nq, nkv, d, amp):
     """anysd_attn_params::aux_cols -- q pre-scaled by scale*log2(e), K carrying 1.0 in padding columns d, d+1 and V
     in column d (what anyedit_b200.unet packs for d = 40): same softmax(q k^T scale) v as the plain contract.  `amp`
-    widens the score range so the in-kernel reference moves many times (rewrites of q's padding columns); keys are
-    sorted by growing norm in the amp = 12 cases so the maximum keeps rising tile after tile.  n_q % 256 == 0 with >= 1024
-    keys runs the paired kernel (two query tiles per CTA, attention_tc5x2_kernel), the rest the one-tile kernel."""
+    widens the score range so the running maximum moves many times; keys are sorted by growing norm in the amp = 12
+    cases so the maximum keeps rising tile after tile."""
     from anyedit_b200.unet import LOG2E, aux_cols_for, head_stride_for
     from oracle import unet_oracle
     assert aux_cols_for(d)
@@ -469,7 +468,7 @@ def test_gemm_epilogue_statistics_and_groupnorm_apply(ops, stats_everywhere):
 
 
 def test_split_k_contractions(ops, stats_everywhere):
-    """Few output tiles + very long K (the 8x8 level's 2560 -> 1280 convs: 40..80 tiles over K = 23040 on 148 SMs): the schedule
+    """Few output tiles + very long K (the 8x8 level's 2560 -> 1280 convs: 40..80 tiles over K = 23040 on 132 SMs): the schedule
     splits K across CTAs; the partial sums are added in split order by whichever unit arrives last, so two runs agree bit for
     bit and the result matches the unsplit arithmetic to fp32 summation-order noise."""
     import ctypes as C
@@ -560,7 +559,7 @@ def test_layernorm_fold_unsupported_is_loud(ops):
 
 def test_gelu_epilogue_accuracy(ops):
     """The GELU of the contraction epilogues (act 2 GEGLU, act 3 nn.GELU) is the exact erf form evaluated as a fitted logistic
-    (gemm_tc5p.cu: p_gelu): |x Phi(x) - kernel| <= 1.2e-5 + fp16 rounding over the whole range, including the saturated tails."""
+    (gemm_wgmma.cu: p_gelu): |x Phi(x) - kernel| <= 1.2e-5 + fp16 rounding over the whole range, including the saturated tails."""
     x = torch.cat([torch.linspace(-12, 12, 64 * 1024 - 6), torch.tensor([-1e4, -60.0, -0.0, 0.0, 60.0, 1e4])]).half()
     A = x.view(-1, 64).cuda()                                  # values pass through an identity contraction
     W = torch.eye(64, dtype=torch.float16, device="cuda")

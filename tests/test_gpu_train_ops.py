@@ -99,8 +99,8 @@ def test_attention_backward(ops, B, heads, nq, nkv, d, self_attn, gated, ln2):
 
 @pytest.mark.parametrize("B,heads,nq,nkv,d,aux", [(2, 3, 256, 256, 40, True), (1, 2, 128, 512, 40, True), (1, 2, 384, 128, 24, False),
                                                   (1, 8, 1024, 1024, 40, True)])
-def test_attention_backward_tcgen05(ops, monkeypatch, B, heads, nq, nkv, d, aux):
-    """The tcgen05 backward (attention_bwd_tc5.cu): the forward hands over its base-2 log-sum-exp (anysd_attn_params::lse), the
+def test_attention_backward_wgmma(ops, monkeypatch, B, heads, nq, nkv, d, aux):
+    """The wgmma backward (attention_wgmma.cu): the forward hands over its base-2 log-sum-exp (anysd_attn_params::lse), the
     backward recomputes P = 2^(s - lse) and forms dS, dQ, dK, dV on the tensor cores.  Checked against autograd, against the
     mma.sync kernels on the same inputs, and the log-sum-exp against torch.logsumexp."""
     from anyedit_b200.unet import head_stride_for
@@ -133,7 +133,7 @@ def test_attention_backward_tcgen05(ops, monkeypatch, B, heads, nq, nkv, d, aux)
     assert float((lse.cpu() - lse_ref).abs().max()) < 2e-3
     dO16 = dO.reshape(B, nq, C).half().cuda().contiguous()
     res = {}
-    for mode in ("tc5", "mma"):
+    for mode in ("wgmma", "mma"):
         if mode == "mma":
             lse_arg = None
         else:
@@ -154,9 +154,9 @@ def test_attention_backward_tcgen05(ops, monkeypatch, B, heads, nq, nkv, d, aux)
             e = rel(g4[..., :d], ref)
             print(f"attention backward {mode} B={B} h={heads} nq={nq} nkv={nkv} d={d} {name}: {e:.2e}")
             assert e < 4e-3, (mode, name, e)
-    assert not torch.equal(res["tc5"][0], res["mma"][0])                          # the two really are different kernels
+    assert not torch.equal(res["wgmma"][0], res["mma"][0])                        # the two really are different kernels
     # frozen K/V, accumulated onto an existing gradient
-    dq2 = res["tc5"][0].clone()
+    dq2 = res["wgmma"][0].clone()
     ops.attention_bwd(q16, k16, v16, dO16, dq2, None, None, B, heads, nq, nkv, d, Cp, Cp, Cp, C, Cp, qk_scale=c, head_stride=hs,
                       out=out, ld_o=C, lse=lse, accumulate_dq=True)
     assert rel(unpad(dq2, nq)[..., :d], 2 * qr.grad) < 4e-3

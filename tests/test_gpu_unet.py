@@ -391,7 +391,7 @@ def test_two_rank_nccl_broadcast_and_shard(tmp_path):
     """2-GPU run (skipped on a 1-GPU box): weights broadcast once over NCCL from rank 0, requests sharded, the two
     ranks' outputs concatenated equal rank 0's unsharded run."""
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs 2 GPUs (gpurun --gpus 2)")
+        pytest.skip("needs 2 GPUs")
     import subprocess
     import sys
     root = os.path.abspath(os.path.join(os.path.dirname(__file__), ".."))

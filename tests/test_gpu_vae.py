@@ -74,7 +74,7 @@ def test_softmax_rows_and_posterior_kernels():
 def test_autoencoder_vs_reference_golden(name):
     """encode -> moments and decode -> image against the reference Encoder / Decoder (+ the 1x1 quant convs): vae_mid has
     the SD ladder at half width (64..512 channels, C = 512 mid attention on the two-contraction path, C = 128 attention on
-    the tcgen05 attention kernel, the right/bottom-padded Downsample); vae_tiny (32..128 channels) runs the decoder on
+    the wgmma attention kernel, the right/bottom-padded Downsample); vae_tiny (32..128 channels) runs the decoder on
     the kernels' fallback tiles."""
     net, g = _build(name)
     img = net.decode(torch.from_numpy(g["z"]).cuda())
