@@ -2,14 +2,21 @@
 // online softmax in fp32 on the accumulator fragment.  Replaces the n x n score tensor of the reference's eager
 // CrossAttention (ldm/modules/attention.py:171-193).
 //
-//   CTA = 128 query rows of one (batch, head), 288 threads: warpgroups 0 and 1 own 64 query rows each, warp 8 is the
-//   TMA producer (Q once, then a 2-stage ring of (K, V) tiles of BKV rows, 128-byte swizzle).
-//   Per kv tile: S [64 x BKV] = Q K^T (both operands in shared memory, K-extent d_ext = ceil16(d)); masked online
-//   softmax in base 2 (a score row lives in the 4 lanes of a quad); P rounded to fp16 and kept in registers as the
-//   A operand of O [64 x d_ext] += P V, V consumed as an MN-major B operand straight from its row-major tile.
+//   CTA = 128 query rows of one (batch, head), 384 threads: warpgroup 0 is the TMA producer (Q once, then a 3-stage ring
+//   of (K, V) tiles of BKV rows, 128-byte swizzle) and hands its registers to consumer warpgroups 1 and 2 (setmaxnreg
+//   24 / 240), which own 64 query rows each.
+//   Per kv tile: S [64 x BKV] = Q K^T (both operands in shared memory, K-extent d_ext = ceil16(d)); online softmax in
+//   base 2 (a score row lives in the 4 lanes of a quad; keys past n_kv masked in the last, partial tile); P rounded to
+//   fp16 and kept in registers as the A operand of O [64 x d_ext] += P V, V consumed as an MN-major B operand straight
+//   from its row-major tile.
+//   Schedule: the products of tile j are S_j and P_{j-1} V_{j-1}, issued back to back; the softmax of S_j runs while
+//   P_{j-1} V_{j-1} is still on the tensor cores.  The two consumer warpgroups take turns issuing (named barriers 1 and
+//   2), so one warpgroup's exponentials run under the other's products.
 //   d % 16 == 8 needs the head stride padded to >= ceil16(d) with zero columns (anyedit_b200.unet packs q/k/v that way).
 //   aux_cols operands (anysd_attn_params::aux_cols) arrive with q pre-scaled by scale * log2(e); their extra padding
-//   columns multiply zeros here, so the same kernel runs them with a unit scale.
+//   columns multiply zeros here, so they run with a unit scale (the UNIT instances: no scale multiply at all).
+//   Exponent arithmetic: p = ex2(round(s * scale_log2) - m) with the maximum m of the rounded scaled scores, and the
+//   denominator summed from the unrounded fp32 p in a fixed order.
 #include <cuda.h>
 #include <math.h>
 #include <stdlib.h>
@@ -19,7 +26,8 @@
 
 namespace anysd {
 
-constexpr int AW_BQ = 128, AW_THREADS = 288, AW_ATOM = 128 * 128, AW_ST = 2;   // Q atom: 128 rows x 64 halves
+constexpr int AW_BQ = 128, AW_ATOM = 128 * 128, AW_ST = 2;     // Q atom: 128 rows x 64 halves; AW_ST: backward ring
+constexpr int AW_THREADS = 384, AW_KV_ST = 3;                  // forward: producer + 2 consumer warpgroups, (K, V) ring
 
 struct AwArgs {
     __half* out;
@@ -65,27 +73,33 @@ __device__ __forceinline__ uint32_t aw_pack(float a, float b) {
     __half2 h = __floats2half2_rn(a, b);
     return *reinterpret_cast<uint32_t*>(&h);
 }
+// Issue turns of the two consumer warpgroups: warpgroup c waits on named barrier 1 + c before it issues its products, and
+// then arrives on the other one's barrier (both barriers count the 256 consumer threads).
+__device__ __forceinline__ void aw_turn_wait(int c) { asm volatile("bar.sync %0, 256;" ::"r"(1 + c) : "memory"); }
+__device__ __forceinline__ void aw_turn_pass(int c) { asm volatile("bar.arrive %0, 256;" ::"r"(2 - c) : "memory"); }
 
 template <int DP, int BKV>
 struct AwCfg {
     static constexpr int NA = (DP + 63) / 64;                 // 64-column atoms per row
     static constexpr int KV_ATOM = BKV * 128;                 // bytes of one [BKV x 64] K or V atom
     static constexpr int STAGE_BYTES = 2 * NA * KV_ATOM;      // K then V
-    static constexpr int SMEM = NA * AW_ATOM + AW_ST * STAGE_BYTES + 1024 + 128;
+    static constexpr int SMEM = NA * AW_ATOM + AW_KV_ST * STAGE_BYTES + 1024 + 128;
+    static_assert(SMEM <= 227 * 1024, "attention (wgmma): shared memory");
 };
 
-template <int DP, int BKV>
+// UNIT: aux_cols operands (q pre-scaled, unit scale), where the scale multiplies below fold away
+template <int DP, int BKV, bool UNIT>
 __global__ void __launch_bounds__(AW_THREADS, 1)
 attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                        const __grid_constant__ CUtensorMap tmV, const AwArgs p) {
     using Cfg = AwCfg<DP, BKV>;
-    constexpr int NA = Cfg::NA, KV_ATOM = Cfg::KV_ATOM;
+    constexpr int NA = Cfg::NA, KV_ATOM = Cfg::KV_ATOM, ST = AW_KV_ST;
     extern __shared__ unsigned char aw_smem_raw[];
     const uint32_t raw = smem_u32(aw_smem_raw);
     const uint32_t base = (raw + 1023u) & ~1023u;              // 128-byte swizzled tiles want 1024-byte alignment
     const uint32_t kv_off = NA * AW_ATOM;
-    const uint32_t bars = base + kv_off + AW_ST * Cfg::STAGE_BYTES;
-    // barriers: 0 q_full | 1.. kv_full | 1 + AW_ST.. kv_empty
+    const uint32_t bars = base + kv_off + ST * Cfg::STAGE_BYTES;
+    // barriers: 0 q_full | 1.. kv_full | 1 + ST.. kv_empty
     auto BAR = [&](int i) { return bars + 8u * i; };
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -97,23 +111,24 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmK) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmV) : "memory");
         aw_init(BAR(0), 1);
-        for (int s = 0; s < AW_ST; ++s) {
+        for (int s = 0; s < ST; ++s) {
             aw_init(BAR(1 + s), 1);
-            aw_init(BAR(1 + AW_ST + s), 8);                     // one arrive per consumer warp
+            aw_init(BAR(1 + ST + s), 8);                        // one arrive per consumer warp
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
 
-    if (warp == 8) {
-        // ===== TMA producer =====
-        if (lane == 0) {
+    if (warp < 4) {
+        // ===== TMA producer warpgroup: one thread issues the loads =====
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 24;" ::: "memory");
+        if (warp == 0 && lane == 0) {
             const int col0 = h * p.hs;
             aw_expect_tx(BAR(0), NA * AW_ATOM);
             for (int a = 0; a < NA; ++a) aw_tma_2d(base + a * AW_ATOM, &tmQ, BAR(0), col0 + a * 64, b * p.n_q + q0);
             for (int j = 0; j < nt; ++j) {
-                const int s = j % AW_ST;
-                aw_wait(BAR(1 + AW_ST + s), (((uint32_t)j / AW_ST) & 1) ^ 1);
+                const int s = j % ST;
+                aw_wait(BAR(1 + ST + s), (((uint32_t)j / ST) & 1) ^ 1);
                 aw_expect_tx(BAR(1 + s), Cfg::STAGE_BYTES);
                 const uint32_t kb = base + kv_off + s * Cfg::STAGE_BYTES, vb = kb + NA * KV_ATOM;
                 for (int a = 0; a < NA; ++a) aw_tma_2d(kb + a * KV_ATOM, &tmK, BAR(1 + s), col0 + a * 64, b * p.n_kv + j * BKV);
@@ -124,50 +139,79 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
     }
 
     // ===== two consumer warpgroups, 64 query rows each; this thread: rows r0 and r0 + 8 of the warp's 16 =====
-    const int wg = warp >> 2, wq = warp & 3, q4 = lane & 3;
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 240;" ::: "memory");
+    const int wg = __shfl_sync(0xffffffffu, (warp >> 2) - 1, 0);   // warp-uniform to the compiler: keeps wgmma unserialized
+    const int wq = warp & 3, q4 = lane & 3;
     const uint32_t qa = base + wg * 64 * 128;
+    const float c = UNIT ? 1.0f : p.scale_log2;                // > 0 (attention_wg_supported)
     float o[DP / 2];
 #pragma unroll
     for (int i = 0; i < DP / 2; ++i) o[i] = 0.f;
     float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
-    aw_wait(BAR(0), 0);
-    for (int j = 0; j < nt; ++j) {
-        const int s = j % AW_ST;
-        aw_wait(BAR(1 + s), ((uint32_t)j / AW_ST) & 1);
-        const uint32_t kb = base + kv_off + s * Cfg::STAGE_BYTES, vb = kb + NA * KV_ATOM;
-        float sc[BKV / 2];
-        wg_fence();
+    float sc[BKV / 2];                                          // S_j, then its exponentials
+    uint32_t pa[BKV / 16][4];                                   // P_{j-1} in the A-operand register layout of m64k16
+    auto issue_s = [&](int j) {                                 // S_j = Q K_j^T
+        const uint32_t kb = base + kv_off + (j % ST) * Cfg::STAGE_BYTES;
 #pragma unroll
         for (int k = 0; k < DP / 16; ++k)
             Wgmma<BKV>::ss(sc, wg_desc(qa + (k >> 2) * AW_ATOM + (k & 3) * 32, 16, 1024),
                            wg_desc(kb + (k >> 2) * KV_ATOM + (k & 3) * 32, 16, 1024), k > 0);
         wg_commit();
-        wg_wait<0>();
+    };
+    auto issue_pv = [&](int j) {                                // O += P_j V_j
+        const uint32_t vb = base + kv_off + (j % ST) * Cfg::STAGE_BYTES + NA * KV_ATOM;
+#pragma unroll
+        for (int kk = 0; kk < BKV / 16; ++kk) Wgmma<DP>::rs_t(o, pa[kk], wg_desc(vb + kk * 2048, KV_ATOM, 1024), 1);
+        wg_commit();
+    };
+    auto release = [&](int j) {                                 // after O += P_j V_j has completed: K/V stage free
+#pragma unroll
+        for (int i = 0; i < DP / 2; ++i) wg_fence_regs(o[i]);
+        __syncwarp();
+        if (lane == 0) aw_arrive(BAR(1 + ST + j % ST));
+    };
+    // online softmax (base 2) of the completed S_j: sc becomes its exponentials, corr the factor of the running sums.
+    // The compiler turns the mask of the last, partial tile into a select per element on every tile; measured on the H100,
+    // a second softmax body without it was slower (larger loop), so the mask stays inline.
+    auto softmax = [&](int j, float (&corr)[2]) {
 #pragma unroll
         for (int i = 0; i < BKV / 2; ++i) wg_fence_regs(sc[i]);
-
-        // ---- scale, mask, online softmax (base 2) ----
         const int kv_left = p.n_kv - j * BKV;
+        if (kv_left < BKV) {                                    // keys past n_kv
+#pragma unroll
+            for (int i = 0; i < BKV / 8; ++i)
+#pragma unroll
+                for (int e = 0; e < 4; ++e)
+                    if (8 * i + 2 * q4 + (e & 1) >= kv_left) sc[4 * i + e] = -INFINITY;
+        }
+        // row maxima of the unscaled scores: c > 0 and rounding is monotone, so max(s) c rounds to the maximum of the rounded s c
         float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
         for (int i = 0; i < BKV / 8; ++i)
 #pragma unroll
-            for (int e = 0; e < 4; ++e) {
-                float v = sc[4 * i + e] * p.scale_log2;
-                if (kv_left < BKV && 8 * i + 2 * q4 + (e & 1) >= kv_left) v = -INFINITY;
-                sc[4 * i + e] = v;
-                mx[e >> 1] = fmaxf(mx[e >> 1], v);
-            }
-        float corr[2];
+            for (int e = 0; e < 4; ++e) mx[e >> 1] = fmaxf(mx[e >> 1], sc[4 * i + e]);
 #pragma unroll
         for (int r = 0; r < 2; ++r) {
             mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
             mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
-            const float m_new = fmaxf(m_run[r], mx[r]);
+            const float m_new = fmaxf(m_run[r], mx[r] * c);
             corr[r] = aw_ex2(m_run[r] - m_new);                // first tile: ex2(-inf) = 0
             m_run[r] = m_new;
             l_run[r] *= corr[r];
         }
+        // p = 2^(round(s c) - m): the scaled score is rounded before the maximum is subtracted (no FFMA), so every p
+        // keeps the bits of scaling the score row first
+#pragma unroll
+        for (int kk = 0; kk < BKV / 16; ++kk) {
+            float* t = sc + 8 * kk;
+#pragma unroll
+            for (int e = 0; e < 8; ++e) t[e] = aw_ex2((UNIT ? t[e] : __fmul_rn(t[e], c)) - m_run[(e >> 1) & 1]);
+            l_run[0] += (t[0] + t[1]) + (t[4] + t[5]);
+            l_run[1] += (t[2] + t[3]) + (t[6] + t[7]);
+        }
+    };
+    // once O += P_{j-1} V_{j-1} has completed: O rescaled to the new row maxima, P_j packed as the next A operand
+    auto rescale_pack = [&](const float (&corr)[2]) {
 #pragma unroll
         for (int i = 0; i < DP / 8; ++i) {
             o[4 * i] *= corr[0];
@@ -175,33 +219,47 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
             o[4 * i + 2] *= corr[1];
             o[4 * i + 3] *= corr[1];
         }
-        // P in the A-operand register layout of m64k16: the S fragment of columns 16 kk .. 16 kk + 15
-        uint32_t pa[BKV / 16][4];
 #pragma unroll
         for (int kk = 0; kk < BKV / 16; ++kk) {
             const float* t = sc + 8 * kk;
-            const float p0 = aw_ex2(t[0] - m_run[0]), p1 = aw_ex2(t[1] - m_run[0]);
-            const float p2 = aw_ex2(t[2] - m_run[1]), p3 = aw_ex2(t[3] - m_run[1]);
-            const float p4 = aw_ex2(t[4] - m_run[0]), p5 = aw_ex2(t[5] - m_run[0]);
-            const float p6 = aw_ex2(t[6] - m_run[1]), p7 = aw_ex2(t[7] - m_run[1]);
-            l_run[0] += (p0 + p1) + (p4 + p5);
-            l_run[1] += (p2 + p3) + (p6 + p7);
-            pa[kk][0] = aw_pack(p0, p1);
-            pa[kk][1] = aw_pack(p2, p3);
-            pa[kk][2] = aw_pack(p4, p5);
-            pa[kk][3] = aw_pack(p6, p7);
+            pa[kk][0] = aw_pack(t[0], t[1]);
+            pa[kk][1] = aw_pack(t[2], t[3]);
+            pa[kk][2] = aw_pack(t[4], t[5]);
+            pa[kk][3] = aw_pack(t[6], t[7]);
         }
-        // ---- O += P V ----
+    };
+
+    // Turn order: warpgroup 0 takes the first turn without waiting, and warpgroup 1 passes no turn after its last one, so
+    // every bar.sync meets exactly one bar.arrive.
+    aw_wait(BAR(0), 0);
+    float corr[2];
+    aw_wait(BAR(1), 0);
+    if (wg == 1) aw_turn_wait(wg);
+    wg_fence();
+    issue_s(0);
+    aw_turn_pass(wg);
+    wg_wait<0>();
+    softmax(0, corr);
+    rescale_pack(corr);
+    for (int j = 1; j < nt; ++j) {
+        aw_wait(BAR(1 + j % ST), ((uint32_t)j / ST) & 1);
+        aw_turn_wait(wg);
         wg_fence();
-#pragma unroll
-        for (int kk = 0; kk < BKV / 16; ++kk) Wgmma<DP>::rs_t(o, pa[kk], wg_desc(vb + kk * 2048, KV_ATOM, 1024), 1);
-        wg_commit();
+        issue_s(j);
+        issue_pv(j - 1);
+        aw_turn_pass(wg);
+        wg_wait<1>();                                           // S_j done; P_{j-1} V_{j-1} still running
+        softmax(j, corr);
         wg_wait<0>();
-#pragma unroll
-        for (int i = 0; i < DP / 2; ++i) wg_fence_regs(o[i]);
-        __syncwarp();
-        if (lane == 0) aw_arrive(BAR(1 + AW_ST + s));           // K/V stage free
+        release(j - 1);
+        rescale_pack(corr);
     }
+    aw_turn_wait(wg);
+    wg_fence();
+    issue_pv(nt - 1);
+    wg_wait<0>();
+    if (wg == 0) aw_turn_pass(wg);
+    release(nt - 1);
 
     // ---- epilogue: O / l -> fp16 -> global ----
     const float g = p.gate ? p.gate[(size_t)b * p.gate_stride] : 1.0f;
@@ -265,6 +323,7 @@ bool attention_wg_supported(const anysd_attn_params* q) {
     if (d_ext > hs && q->heads > 1) return false;              // K-extent would reach into the next head's columns
     if (q->d % 8 != 0 || d_ext > 160) return false;
     if (q->aux_cols && (q->d % 16 != 8 || hs < q->d + 8)) return false;
+    if (!q->aux_cols && !(q->scale > 0.f)) return false;       // the kernel takes the row maximum before scaling
     if (q->ld_q % 8 || q->ld_k % 8 || q->ld_v % 8 || q->ld_o % 8) return false;
     if (((uintptr_t)q->q % 16) || ((uintptr_t)q->k % 16) || ((uintptr_t)q->v % 16) || ((uintptr_t)q->out % 16)) return false;
     // batches must be stacked rows of one matrix (what the UNet produces): batch stride = n * ld
@@ -296,7 +355,9 @@ static int aw_launch(const anysd_attn_params* q, const AwArgs& a, cudaStream_t s
     cudaGetDevice(&dev);
     dev &= 63;
     if (!done[dev]) {
-        cudaError_t e = cudaFuncSetAttribute(attention_wgmma_kernel<DP, BKV>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM);
+        cudaError_t e = cudaFuncSetAttribute(attention_wgmma_kernel<DP, BKV, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM);
+        if (e == cudaSuccess)
+            e = cudaFuncSetAttribute(attention_wgmma_kernel<DP, BKV, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM);
         if (e != cudaSuccess) {
             set_error("attention (wgmma): smem opt-in failed: %s", cudaGetErrorString(e));
             return ANYSD_ECUDA;
@@ -304,7 +365,8 @@ static int aw_launch(const anysd_attn_params* q, const AwArgs& a, cudaStream_t s
         done[dev] = true;
     }
     dim3 grid(cdiv(q->n_q, AW_BQ), q->heads, q->B);
-    attention_wgmma_kernel<DP, BKV><<<grid, AW_THREADS, Cfg::SMEM, st>>>(tmQ, tmK, tmV, a);
+    if (q->aux_cols) attention_wgmma_kernel<DP, BKV, true><<<grid, AW_THREADS, Cfg::SMEM, st>>>(tmQ, tmK, tmV, a);
+    else attention_wgmma_kernel<DP, BKV, false><<<grid, AW_THREADS, Cfg::SMEM, st>>>(tmQ, tmK, tmV, a);
     return check_launch("attention (wgmma)");
 }
 
