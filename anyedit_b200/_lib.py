@@ -28,6 +28,7 @@ class GemmParams(C.Structure):
         ("splitk_workspace", C.c_void_p), ("splitk_workspace_bytes", C.c_size_t),
         ("splitk_counters", C.c_void_p), ("splitk_counters_bytes", C.c_size_t),
         ("row_stats", C.c_void_p), ("ln_stats", C.c_void_p), ("ln_colsum", C.c_void_p), ("ln_eps", C.c_float),
+        ("col_scale", C.c_void_p),
     ]
 
 

@@ -173,14 +173,24 @@ class ControlNet(UNetModel):
 
 
 class ControlDenoiser(LatentDenoiser):
-    """``ControlLDM.apply_model`` (cldm.py:328-340) for the samplers: ``cond = {"c_concat": [hint], "c_crossattn": [text]}``."""
+    """``ControlLDM.apply_model`` (cldm.py:328-340) for the samplers: ``cond = {"c_concat": [hint], "c_crossattn": [text]}``.
+    ``cond_stage_model`` (e.g. ``encoders.FrozenDinoV2Encoder``): what ``get_learned_conditioning`` runs."""
 
-    def __init__(self, unet, control_model, only_mid_control=False, control_scales=None, **kwargs):
+    def __init__(self, unet, control_model, only_mid_control=False, control_scales=None, cond_stage_model=None, **kwargs):
         super().__init__(unet, "crossattn", **kwargs)
         assert isinstance(control_model, ControlNet)
         self.control_model = control_model
         self.only_mid_control = only_mid_control
         self.control_scales = list(control_scales) if control_scales is not None else [1.0] * 13
+        self.cond_stage_model = cond_stage_model
+
+    def get_learned_conditioning(self, c):
+        """LatentDiffusion.get_learned_conditioning (ddpm.py) without a ``cond_stage_forward``: the model's ``encode`` when it
+        has one, else its call -- visual_reference_tool.py:203-205 turns the reference image (and zeros) into c_crossattn."""
+        m = self.cond_stage_model
+        if m is None:
+            raise RuntimeError("ControlDenoiser: constructed without a cond_stage_model")
+        return m.encode(c) if callable(getattr(m, "encode", None)) else m(c)
 
     @property
     def graph_safe(self):

@@ -22,10 +22,15 @@ extern "C" int anysd_gemm_f16(const anysd_gemm_params* p, anysd_stream_t stream)
                   "gemm: K=%d and ldw=%d must be multiples of 8 with ldw >= K", p->K, p->ldw);
     ANYSD_REQUIRE(((uintptr_t)p->A % 16) == 0 && ((uintptr_t)p->W % 16) == 0, ANYSD_EINVAL,
                   "gemm: A and W must be 16-byte aligned");
-    ANYSD_REQUIRE(p->act >= 0 && p->act <= 4, ANYSD_EINVAL, "gemm: bad act %d", p->act);
+    ANYSD_REQUIRE(p->act >= 0 && p->act <= 5, ANYSD_EINVAL, "gemm: bad act %d", p->act);
     ANYSD_REQUIRE(p->out_dtype == ANYSD_F16 || p->out_dtype == ANYSD_F32, ANYSD_EINVAL, "gemm: bad out dtype");
-    const int n_out = (p->act == 2) ? p->N / 2 : p->N;
-    ANYSD_REQUIRE(p->act != 2 || p->N % 2 == 0, ANYSD_EINVAL, "gemm: GEGLU needs an even N");
+    const bool glu = p->act == 2 || p->act == 5;
+    const int n_out = glu ? p->N / 2 : p->N;
+    ANYSD_REQUIRE(!glu || p->N % 2 == 0, ANYSD_EINVAL, "gemm: GEGLU / SwiGLU needs an even N");
+    ANYSD_REQUIRE(p->act != 5 || !p->conv, ANYSD_EUNSUPPORTED, "gemm: SwiGLU (act 5) is for dense contractions only");
+    ANYSD_REQUIRE(!p->col_scale || (p->act == 0 && !p->conv && !p->stats && !p->row_stats && !p->ln_stats), ANYSD_EUNSUPPORTED,
+                  "gemm: col_scale needs act = 0, a dense contraction and no GroupNorm / row / LayerNorm statistics (act=%d conv=%d)",
+                  p->act, p->conv);
     ANYSD_REQUIRE(p->ldo >= n_out, ANYSD_EINVAL, "gemm: ldo=%d < %d output columns", p->ldo, n_out);
     ANYSD_REQUIRE(!p->residual || p->ldr >= n_out, ANYSD_EINVAL, "gemm: ldr too small");
     ANYSD_REQUIRE(!p->rowadd || (p->rows_per_batch > 0 && p->ld_rowadd >= p->N), ANYSD_EINVAL,

@@ -2,7 +2,8 @@
 // cp.async pipeline with XOR-swizzled shared memory.  One template serves nn.Linear / 1x1 conv
 // (dense A rows) and 3x3 conv (A gathered from the NHWC image: stride 1|2, optional nearest-x2
 // upsample folded into the gather coordinates, zero-fill halo through cp.async src-size 0).
-// Epilogue (fp32): + bias[n] + rowadd[m / rows_per_batch, n] -> SiLU | GEGLU -> + residual -> fp16|fp32.
+// Epilogue (fp32): + bias[n] + rowadd[m / rows_per_batch, n] -> x col_scale[n] -> activation | GEGLU | SwiGLU -> + residual
+// -> fp16|fp32.
 //
 // This is the correctness baseline the wgmma kernel (gemm_wgmma.cu) is validated against;
 // the dispatch in anysd_gemm_f16 prefers wgmma wherever its shape constraints hold.
@@ -27,6 +28,7 @@ struct GemmArgs {
     int act, out_f16;
     // conv
     int H, Wd, Cin, Ho, Wo, stride, up;
+    const float* col_scale;
 };
 
 // byte offset of 16-byte chunk `cc` (0..3) of row `r` inside a [rows][32 halves] tile
@@ -177,8 +179,12 @@ __global__ void __launch_bounds__(GEMM_THREADS, 2) gemm_mma_kernel(const GemmArg
                     v0 += radd[n];
                     if (has1) v1 += radd[n + 1];
                 }
-                if (p.act == 2) {  // GEGLU: (a, gate) interleaved -> one output column n/2
-                    float o = v0 * gelu_erf_f(v1);
+                if (p.col_scale) {
+                    v0 *= p.col_scale[n];
+                    if (has1) v1 *= p.col_scale[n + 1];
+                }
+                if (p.act == 2 || p.act == 5) {  // GEGLU / SwiGLU: (a, gate) interleaved -> one output column n/2
+                    float o = v0 * (p.act == 5 ? silu_f(v1) : gelu_erf_f(v1));
                     const int no = n >> 1;
                     if (p.residual) o += __half2float(p.residual[(size_t)m * p.ldr + no]);
                     if (p.out_f16)
@@ -227,6 +233,7 @@ int launch_gemm_mma(const anysd_gemm_params* q, cudaStream_t st) {
     a.rows_per_batch = q->rows_per_batch > 0 ? q->rows_per_batch : 1;
     a.act = q->act;
     a.out_f16 = q->out_dtype == ANYSD_F16;
+    a.col_scale = q->col_scale;
     a.H = q->H; a.Wd = q->Wd; a.Cin = q->Cin; a.stride = q->stride; a.up = q->upsample;
     a.Ho = a.Wo = 0;
     if (q->conv) {

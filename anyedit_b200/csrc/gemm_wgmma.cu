@@ -7,8 +7,9 @@
 //     map's out-of-bounds fill), a ring of STAGES x (16 KB A + BN x 128 B of B), 128-byte swizzle;
 //   * warpgroups 1 and 2: 64 rows of the tile each, wgmma m64nBNk16 into register accumulators while the producer
 //     already streams the next unit's operands; the epilogue works on the accumulator fragment in place: bias or
-//     folded LayerNorm, time-embedding row add, SiLU / GELU / QuickGELU / GEGLU, residual, fp16 or fp32 stores,
-//     GroupNorm statistics (per 32-row slab and channel) and LayerNorm row statistics (per 64-column slab) of the output.
+//     folded LayerNorm, time-embedding row add, per-column scale (LayerScale), SiLU / GELU / QuickGELU / GEGLU / SwiGLU,
+//     residual, fp16 or fp32 stores, GroupNorm statistics (per 32-row slab and channel) and LayerNorm row statistics (per
+//     64-column slab) of the output.
 #include <cuda.h>
 #include <stdlib.h>
 
@@ -25,6 +26,7 @@ struct GCfg {
     static constexpr int STAGE_BYTES = G_A_BYTES + BN * G_BK * 2;
     static constexpr int RED_BYTES = 8 * BN * 8;    // per consumer warp: BN x {sum, sum of squares} (GroupNorm statistics)
     static constexpr int PAR_BYTES = 2 * 2 * BN * 4;  // per consumer warpgroup: the unit's bias and folded-LayerNorm column sums
+                                                      // (or column scales: the two are never combined)
     static constexpr int FIT = (212 * 1024 - RED_BYTES - PAR_BYTES) / STAGE_BYTES;
     static constexpr int STAGES = FIT > 6 ? 6 : FIT;
     static constexpr int SMEM = STAGES * STAGE_BYTES + RED_BYTES + PAR_BYTES + 1024 + 256;
@@ -60,6 +62,7 @@ struct GArgs {
     const float* ln_colsum;                  // [N]
     int ln_slabs;
     float ln_eps, ln_inv_k;
+    const float* col_scale;                  // [N] or NULL (anysd_gemm_params::col_scale; act 0, no LayerNorm fold)
 };
 
 __device__ __forceinline__ void g_bar_init(uint32_t bar, uint32_t count) {
@@ -200,10 +203,15 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     const int q4 = lane & 3;
     const bool ln_in = !CONV && p.ln_stats != nullptr;
     const bool row_st = !CONV && p.row_stats != nullptr;
-    // the unit's bias / column sums reach the epilogue through shared memory, loaded before the mainloop: read straight from
-    // global memory inside the epilogue they would cost one L2 round trip per 8-column step
+    // SwiGLU and the column scale are dense only (anysd_gemm_f16 refuses them on convs)
+    const bool swiglu = !CONV && p.act == 5;
+    const bool glu = p.act == 2 || swiglu;                // GEGLU / SwiGLU: (a, gate) column pairs, N / 2 outputs
+    const bool col_sc = !CONV && p.col_scale != nullptr;
+    // the unit's bias / column sums (or column scales) reach the epilogue through shared memory, loaded before the mainloop:
+    // read straight from global memory inside the epilogue they would cost one L2 round trip per 8-column step
     float* s_bias = par + wg * 2 * BN;
     float* s_cs = s_bias + BN;
+    const float* colv = ln_in ? p.ln_colsum : (col_sc ? p.col_scale : nullptr);   // what s_cs holds (never both)
     const int wtid = threadIdx.x & 127;
     float acc[BN / 2];
     uint32_t g = 0;
@@ -218,7 +226,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         for (int r = 0; r < 2; ++r) {
             const int j = wtid + 128 * r, col = n0 + j;
             pb[r] = (j < BN && col < p.N && p.bias != nullptr) ? __ldg(p.bias + col) : 0.f;
-            pc[r] = (j < BN && col < p.N && ln_in) ? __ldg(p.ln_colsum + col) : 0.f;
+            pc[r] = (j < BN && col < p.N && colv != nullptr) ? __ldg(colv + col) : 0.f;
         }
 #pragma unroll
         for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
@@ -327,7 +335,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                 }
             }
         }
-        auto store2 = [&](int h, int ocol, float a, float b) {      // GEGLU outputs (residual read here)
+        auto store2 = [&](int h, int ocol, float a, float b) {      // GEGLU / SwiGLU outputs (residual read here)
             if (valid[h]) {
                 if (p.residual != nullptr) {
                     const float2 r = __half22float2(*reinterpret_cast<const __half2*>(p.residual + pix[h] * p.ldr + ocol));
@@ -370,7 +378,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                     ra[u][h] = (in && p.rowadd != nullptr)
                                    ? __ldg(reinterpret_cast<const float2*>(p.rowadd + (size_t)img[h] * p.ld_rowadd + cw))
                                    : make_float2(0.f, 0.f);
-                    rr[u][h] = (in && valid[h] && p.residual != nullptr && p.act != 2)
+                    rr[u][h] = (in && valid[h] && p.residual != nullptr && !glu)
                                    ? *reinterpret_cast<const __half2*>(p.residual + pix[h] * p.ldr + cw)
                                    : __floats2half2_rn(0.f, 0.f);
                 }
@@ -401,12 +409,21 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                 v[h][0] += ra[u][h].x;
                 v[h][1] += ra[u][h].y;
             }
-            if (p.act == 2) {
-                // GEGLU: (a, gate) column pairs -> one output at column col / 2; neighbouring lanes swap so that each
-                // stores two adjacent outputs (the even lane of row rl0, the odd lane of row rl0 + 8)
+            if (col_sc) {                                 // LayerScale: s_n (acc + bias_n + rowadd); s_cs holds s here
+                const float2 sc = *reinterpret_cast<const float2*>(s_cs + 8 * i + 2 * q4);
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    v[h][0] *= sc.x;
+                    v[h][1] *= sc.y;
+                }
+            }
+            if (glu) {
+                // GEGLU / SwiGLU: (a, gate) column pairs -> one output at column col / 2; neighbouring lanes swap so that
+                // each stores two adjacent outputs (the even lane of row rl0, the odd lane of row rl0 + 8)
                 float gv[2];
 #pragma unroll
-                for (int h = 0; h < 2; ++h) gv[h] = v[h][0] * (p.out_f16 ? p_gelu(v[h][1]) : gelu_erf_f(v[h][1]));
+                for (int h = 0; h < 2; ++h)
+                    gv[h] = v[h][0] * (swiglu ? silu_f(v[h][1]) : (p.out_f16 ? p_gelu(v[h][1]) : gelu_erf_f(v[h][1])));
                 const float recv = __shfl_xor_sync(0xffffffffu, (lane & 1) ? gv[0] : gv[1], 1);
                 const int h = lane & 1;
                 const int ocol = (col >> 1) - h;
@@ -639,7 +656,7 @@ static void p_conv_patch(const anysd_gemm_params* q, int* Ho, int* Wo, int* BW, 
 // GroupNorm statistics from the epilogue: possible when every 32-row slab of the output lies inside one image and the
 // conv patches tile the image exactly.  Returns the slabs per image (rows_per_batch / 32), 0 when not possible.
 int wg_stats_slabs(const anysd_gemm_params* q) {
-    if (q->act == 2 || q->out_dtype != ANYSD_F16) return 0;
+    if (q->act == 2 || q->act == 5 || q->out_dtype != ANYSD_F16) return 0;
     const int hw = q->rows_per_batch;
     if (hw <= 0 || hw % 32 != 0 || q->M % hw != 0) return 0;
     if (q->conv) {
@@ -659,7 +676,9 @@ int wg_stats_slabs(const anysd_gemm_params* q) {
 // ANYSD_GEMM_SPLITK=0|n forces a count (experiments).
 static int p_geometry_splits(const anysd_gemm_params* q, int num_kb) {
     static const char* force_sk = getenv("ANYSD_GEMM_SPLITK");
-    if (q->act == 2 || q->out_dtype != ANYSD_F16 || q->row_stats != nullptr || q->ln_stats != nullptr) return 1;
+    if (q->act == 2 || q->act == 5 || q->out_dtype != ANYSD_F16 || q->row_stats != nullptr || q->ln_stats != nullptr ||
+        q->col_scale != nullptr)
+        return 1;
     int rows_per_image = q->rows_per_batch;
     if (q->conv) {
         int Ho, Wo, BW, BH, NB;
@@ -736,15 +755,16 @@ static const char* wg_ln_unsupported(const anysd_gemm_params* q) {
         if (q->bias == nullptr || q->ln_colsum == nullptr) return "folded LayerNorm needs bias (beta W^T + b) and ln_colsum";
         if (((uintptr_t)q->ln_stats % 8) || ((uintptr_t)q->ln_colsum % 16)) return "ln_stats / ln_colsum misaligned";
         if (q->N % 32 != 0) return "folded LayerNorm needs N % 32 == 0";
-        if (q->act != 0 && q->act != 1 && q->act != 2) return "folded LayerNorm: act must be 0, 1 or 2";
+        if (q->act != 0 && q->act != 1 && q->act != 2 && q->act != 5) return "folded LayerNorm: act must be 0, 1, 2 or 5";
     }
     return nullptr;
 }
 
 bool wg_supported(const anysd_gemm_params* q) {
     if (q->N % 8 != 0 || q->K % 8 != 0) return false;
-    if (q->act == 2 && q->N % 16 != 0) return false;
-    const int n_out = q->act == 2 ? q->N / 2 : q->N;
+    const bool glu = q->act == 2 || q->act == 5;
+    if (glu && q->N % 16 != 0) return false;
+    const int n_out = glu ? q->N / 2 : q->N;
     if (((uintptr_t)q->out % 16) || q->ldo % 8 != 0 || n_out % 4 != 0) return false;
     if (q->residual && (((uintptr_t)q->residual % 16) || q->ldr % 8 != 0)) return false;
     if (q->bias && ((uintptr_t)q->bias % 16)) return false;
@@ -810,13 +830,14 @@ int launch_gemm_wg(const anysd_gemm_params* q, cudaStream_t st) {
     a.ln_slabs = q->K / 64;
     a.ln_eps = q->ln_eps;
     a.ln_inv_k = 1.0f / (float)q->K;
+    a.col_scale = q->col_scale;                       // combinations anysd_gemm_f16 refuses never reach here
     if (q->row_stats != nullptr || q->ln_stats != nullptr) {
         const char* why = wg_ln_unsupported(q);
         if (why) {
             set_error("gemm: LayerNorm fold / row statistics: %s (M=%d N=%d K=%d act=%d)", why, q->M, q->N, q->K, q->act);
             return ANYSD_EUNSUPPORTED;
         }
-        if (q->stats != nullptr || q->act >= 3) {
+        if (q->stats != nullptr || q->act == 3 || q->act == 4) {
             set_error("gemm: LayerNorm fold / row statistics cannot be combined with GroupNorm statistics or GELU epilogues");
             return ANYSD_EUNSUPPORTED;
         }

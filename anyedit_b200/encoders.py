@@ -11,6 +11,9 @@ before the denoising loop.
   ``Resampler``                     AnyEdit_Collection/other_modules/ip_adapter/resampler.py:81-147 (perceiver attention of 16
                                     latent queries over [image tokens ; latents], FeedForward, proj_out + LayerNorm).
   ``ImageProjModel``                ip_adapter/ip_adapter.py:28-46.
+  ``FrozenDinoV2Encoder``           ldm/modules/encoders/modules.py:279-315, AnyDoor's ``cond_stage_model``: ImageNet normalisation
+                                    (folded into the patch embedding), DINOv2 ViT-g/14 (``Dinov2Model``: 40 pre-LN blocks, SwiGLU
+                                    MLP and LayerScale in the contraction epilogues, hub key names), Linear(1536, 1024) projector.
 
 The arithmetic of the two CLIP towers lives in a third-party dependency of the reference (``transformers``, unpinned in
 requirements.txt; 5.5 is what this image has): the golden vectors are generated from that library's own modules with seeded
@@ -19,6 +22,7 @@ GELU / residual fused in the epilogue, the wgmma attention kernel for the vision
 causal attention kernel for the 77 text tokens.  Tokenisation (vocabulary files) is outside the path: the text tower takes
 token ids (or a caller-supplied tokenizer).  No eager-PyTorch math, no CPU fallback.
 """
+import re
 import types
 
 import torch
@@ -89,7 +93,9 @@ def _pack_layers(layers, dev):
 
 
 def _run_layers(packed, h, B, n, heads, act, eps, causal, keep_hidden=False, n_run=None):
-    """CLIPEncoder.forward: pre-LN residual blocks on the token matrix h [B*n, D] fp16.  Returns (h, [hidden states])."""
+    """CLIPEncoder.forward: pre-LN residual blocks on the token matrix h [B*n, D] fp16.  Returns (h, [hidden states]).
+    A layer with "ls1" / "ls2" (fp32 [D]) scales its attention / MLP branch by them (LayerScale) in the epilogue that adds
+    the residual; act 5 (SwiGLU) halves the width of the first MLP contraction (the DINOv2 blocks)."""
     M, D = h.shape
     d = D // heads
     dev = h.device
@@ -105,13 +111,13 @@ def _run_layers(packed, h, B, n, heads, act, eps, causal, keep_hidden=False, n_r
         else:
             ops.attention(qkv, qkv[:, D:], qkv[:, 2 * D:], a, B, heads, n, n, d, 3 * D, 3 * D, 3 * D, D)
         h2 = torch.empty_like(h)
-        ops.gemm(a, L["o_w"], h2, bias=L["o_b"], residual=h)
+        ops.gemm(a, L["o_w"], h2, bias=L["o_b"], residual=h, col_scale=L.get("ls1"))
         ln2 = torch.empty_like(h)
         ops.layernorm(h2, L["ln2"][0], L["ln2"][1], ln2, eps)
-        f1 = torch.empty(M, L["fc1_w"].shape[0], dtype=torch.float16, device=dev)
+        f1 = torch.empty(M, L["fc1_w"].shape[0] // (2 if act == 5 else 1), dtype=torch.float16, device=dev)
         ops.gemm(ln2, L["fc1_w"], f1, bias=L["fc1_b"], act=act)
         h = torch.empty_like(h2)
-        ops.gemm(f1, L["fc2_w"], h, bias=L["fc2_b"], residual=h2)
+        ops.gemm(f1, L["fc2_w"], h, bias=L["fc2_b"], residual=h2, col_scale=L.get("ls2"))
         if keep_hidden:
             hidden.append(h)
     return h, hidden
@@ -306,6 +312,228 @@ class CLIPVisionModelWithProjection(_Packable):
         ops.gemm(pooled, P["proj_w"], embeds)
         hs = tuple(t.view(B, n, D).float() for t in hidden) if output_hidden_states else None
         return types.SimpleNamespace(image_embeds=embeds, last_hidden_state=h.view(B, n, D).float(), hidden_states=hs)
+
+
+# ---- DINOv2 ViT-g/14: AnyDoor's reference-image encoder -------------------------------------------------------------------------
+IMAGENET_MEAN, IMAGENET_STD = (0.485, 0.456, 0.406), (0.229, 0.224, 0.225)
+
+
+def dinov2_pos_table(pos_embed, gh, gw, interpolate_offset=0.1):
+    """``DinoVisionTransformer.interpolate_pos_encoding``: the position table trained on an m x m grid ([1, 1 + m*m, D]) resized
+    bicubically to gh x gw patches -> fp32 [1 + gh*gw, D] (class slot first).  Offset 0.1 is the published hub form
+    (``scale_factor=((gh + 0.1) / m, (gw + 0.1) / m)``); 0.0 the ``size=(gh, gw)`` form of transformers' ``Dinov2Embeddings``.
+    Both return the table unchanged on its own square grid."""
+    pos = pos_embed.detach().float().cpu().reshape(-1, pos_embed.shape[-1])
+    m = int(round((pos.shape[0] - 1) ** 0.5))
+    assert m * m == pos.shape[0] - 1, "the position table must cover a square grid plus the class slot"
+    if gh == m and gw == m:
+        return pos
+    grid = pos[1:].reshape(1, m, m, -1).permute(0, 3, 1, 2)
+    if interpolate_offset:
+        kw = {"scale_factor": ((gh + interpolate_offset) / m, (gw + interpolate_offset) / m)}
+    else:
+        kw = {"size": (gh, gw)}
+    g = torch.nn.functional.interpolate(grid, mode="bicubic", align_corners=False, **kw)
+    assert tuple(g.shape[-2:]) == (gh, gw)
+    return torch.cat([pos[:1], g.permute(0, 2, 3, 1).reshape(gh * gw, -1)], 0)
+
+
+# transformers ``Dinov2Model`` name -> hub name.  attention.attention.{query,key,value} are fused (rows q ; k ; v) into attn.qkv.
+_HF_TOP = (("embeddings.cls_token", "cls_token"), ("embeddings.mask_token", "mask_token"),
+           ("embeddings.position_embeddings", "pos_embed"), ("embeddings.patch_embeddings.projection.", "patch_embed.proj."),
+           ("layernorm.", "norm."))
+_HF_BLOCK = (("norm1.", "norm1."), ("attention.output.dense.", "attn.proj."), ("layer_scale1.lambda1", "ls1.gamma"),
+             ("norm2.", "norm2."), ("mlp.weights_in.", "mlp.w12."), ("mlp.weights_out.", "mlp.w3."), ("layer_scale2.lambda1", "ls2.gamma"))
+_QKV = ("query", "key", "value")
+
+
+def _rename(k, table):
+    for a, b in table:
+        if k.startswith(a):
+            return b + k[len(a):]
+    raise KeyError(f"no DINOv2 key mapping for {k!r}")
+
+
+def dinov2_from_transformers(sd):
+    """State dict of transformers' ``Dinov2Model(use_swiglu_ffn=True)`` -> the hub names ``Dinov2Model`` here loads."""
+    out = {}
+    for k, v in sd.items():
+        m = re.fullmatch(r"encoder\.layer\.(\d+)\.(.*)", k)
+        if m is None:
+            out[_rename(k, _HF_TOP)] = v
+        elif m.group(2).startswith("attention.attention."):
+            leaf = m.group(2).rsplit(".", 1)[1]
+            if m.group(2).startswith("attention.attention.query."):
+                pre = f"encoder.layer.{m.group(1)}.attention.attention."
+                out[f"blocks.{m.group(1)}.attn.qkv.{leaf}"] = torch.cat([sd[f"{pre}{n}.{leaf}"] for n in _QKV], 0)
+        else:
+            out[f"blocks.{m.group(1)}.{_rename(m.group(2), _HF_BLOCK)}"] = v
+    return out
+
+
+def dinov2_to_transformers(sd):
+    """Inverse of ``dinov2_from_transformers``."""
+    out = {}
+    for k, v in sd.items():
+        m = re.fullmatch(r"blocks\.(\d+)\.(.*)", k)
+        if m is None:
+            out[_rename(k, tuple((b, a) for a, b in _HF_TOP))] = v
+        elif m.group(2).startswith("attn.qkv."):
+            leaf = m.group(2).rsplit(".", 1)[1]
+            for n, t in zip(_QKV, v.chunk(3, 0)):
+                out[f"encoder.layer.{m.group(1)}.attention.attention.{n}.{leaf}"] = t
+        else:
+            out[f"encoder.layer.{m.group(1)}.{_rename(m.group(2), tuple((b, a) for a, b in _HF_BLOCK))}"] = v
+    return out
+
+
+class _LayerScale(nn.Module):
+    def __init__(self, d):
+        super().__init__()
+        self.gamma = nn.Parameter(torch.ones(d))
+
+
+class _DinoBlock(nn.Module):
+    """Hub ``NestedTensorBlock`` parameter holder: norm1, attn.{qkv, proj}, ls1, norm2, mlp.{w12, w3} (SwiGLUFFNFused), ls2."""
+
+    def __init__(self, d, hidden):
+        super().__init__()
+        self.norm1 = _Param((d,), kind="norm")
+        self.attn = nn.Module()
+        self.attn.qkv, self.attn.proj = _Param((3 * d, d)), _Param((d, d))
+        self.ls1 = _LayerScale(d)
+        self.norm2 = _Param((d,), kind="norm")
+        self.mlp = nn.Module()
+        self.mlp.w12, self.mlp.w3 = _Param((2 * hidden, d)), _Param((d, hidden))
+        self.ls2 = _LayerScale(d)
+
+
+class Dinov2Model(_Packable):
+    """DINOv2 ``DinoVisionTransformer`` with the SwiGLU MLP (hub ``dinov2_vitg14``) under the hub's parameter names.
+    ``config``: dict or transformers ``Dinov2Config`` (hidden_size, num_hidden_layers, num_attention_heads, mlp_ratio, image_size
+    = the resolution of the position table, patch_size, layer_norm_eps); the defaults are ViT-g/14.  ``interpolate_offset``:
+    see ``dinov2_pos_table``.  ``pixel_mean`` / ``pixel_std`` (per channel): an input normalisation folded into the packed
+    patch embedding.  ``forward_features(x)`` -> {"x_norm_clstoken": [B, D], "x_norm_patchtokens": [B, gh*gw, D]} fp32."""
+
+    def __init__(self, config=None, interpolate_offset=0.1, pixel_mean=None, pixel_std=None):
+        super().__init__()
+        self.config = c = _cfg(config if config is not None else {}, hidden_size=1536, num_hidden_layers=40, num_attention_heads=24,
+                               mlp_ratio=4, image_size=518, patch_size=14, num_channels=3, layer_norm_eps=1e-6, use_swiglu_ffn=True)
+        if not c.use_swiglu_ffn:
+            raise NotImplementedError("Dinov2Model: only the SwiGLU MLP of ViT-g/14 is implemented")
+        D, p = c.hidden_size, c.patch_size
+        hidden = (int(int(D * c.mlp_ratio) * 2 / 3) + 7) // 8 * 8     # SwiGLUFFNFused: 6144 -> 4096 for ViT-g
+        m = c.image_size // p
+        self.interpolate_offset, self.pixel_mean, self.pixel_std = interpolate_offset, pixel_mean, pixel_std
+        self.cls_token = nn.Parameter(torch.zeros(1, 1, D))
+        self.pos_embed = nn.Parameter(torch.randn(1, m * m + 1, D) * 0.02)
+        self.mask_token = nn.Parameter(torch.zeros(1, D))           # masked pre-training only; loaded, never used
+        self.patch_embed = nn.Module()
+        self.patch_embed.proj = _Param((D, c.num_channels, p, p), kind="conv")
+        self.blocks = nn.ModuleList([_DinoBlock(D, hidden) for _ in range(c.num_hidden_layers)])
+        self.norm = _Param((D,), kind="norm")
+
+    def _build_pack(self, dev):
+        c, D, p = self.config, self.config.hidden_size, self.config.patch_size
+        k = c.num_channels * p * p
+        kp = (k + 7) // 8 * 8
+        w = self.patch_embed.proj.weight.detach().double().cpu().reshape(D, c.num_channels, p * p)
+        b = self.patch_embed.proj.bias.detach().double().cpu()
+        if self.pixel_mean is not None:              # conv((x - mean) / std) = conv with W / std, bias b - sum W mean / std
+            mean = torch.tensor(self.pixel_mean, dtype=torch.float64)[None, :, None]
+            std = torch.tensor(self.pixel_std, dtype=torch.float64)[None, :, None]
+            b = b - (w * (mean / std)).sum((1, 2))
+            w = w / std
+        wp = torch.zeros(D, kp, dtype=torch.float64)
+        wp[:, :k] = w.reshape(D, k)
+        layers = []
+        for L in self.blocks:
+            w12, b12 = L.mlp.w12.weight, L.mlp.w12.bias
+            hd = w12.shape[0] // 2
+            # act 5 takes rows (a_j, gate_j); the hub computes silu(x1) * x2 with x1, x2 = w12(x).chunk(2): a = x2, gate = x1
+            perm = torch.stack([torch.arange(hd, 2 * hd), torch.arange(hd)], 1).reshape(-1).to(w12.device)
+            layers.append({"ln1": (_f(L.norm1.weight, dev), _f(L.norm1.bias, dev)), "ln2": (_f(L.norm2.weight, dev), _f(L.norm2.bias, dev)),
+                           "qkv_w": _h(L.attn.qkv.weight, dev), "qkv_b": _f(L.attn.qkv.bias, dev),
+                           "o_w": _h(L.attn.proj.weight, dev), "o_b": _f(L.attn.proj.bias, dev), "ls1": _f(L.ls1.gamma, dev),
+                           "fc1_w": _h(w12[perm], dev), "fc1_b": _f(b12[perm], dev),
+                           "fc2_w": _h(L.mlp.w3.weight, dev), "fc2_b": _f(L.mlp.w3.bias, dev), "ls2": _f(L.ls2.gamma, dev)})
+        return {"patch_w": _h(wp, dev), "patch_b": _f(b, dev), "kp": kp, "layers": layers,
+                "norm": (_f(self.norm.weight, dev), _f(self.norm.bias, dev)), "pos": {}}
+
+    def _pos(self, P, gh, gw):
+        """(class token + its position, fp16 [D]; patch positions, fp16 [gh*gw, D]) for one grid, built once per pack."""
+        if (gh, gw) not in P["pos"]:
+            dev = P["patch_w"].device
+            t = dinov2_pos_table(self.pos_embed, gh, gw, self.interpolate_offset).to(dev)
+            cls = self.cls_token.detach().float().reshape(-1) + t[0]
+            P["pos"][(gh, gw)] = (cls.half().contiguous(), t[1:].half().contiguous())
+        return P["pos"][(gh, gw)]
+
+    def normed_tokens(self, x):
+        """-> (fp16 [B * (1 + gh*gw), D] = the final LayerNorm of every token, class token first per image; B; 1 + gh*gw)."""
+        P, c = self._packed(), self.config
+        dev = P["patch_w"].device
+        x = x.to(dev)
+        B, Cc, H, W = x.shape
+        p, D = c.patch_size, c.hidden_size
+        assert Cc == c.num_channels and H % p == 0 and W % p == 0, f"expected [B, {c.num_channels}, H, W] with H, W multiples of {p}"
+        gh, gw = H // p, W // p
+        npatch, n = gh * gw, gh * gw + 1
+        cls, pos = self._pos(P, gh, gw)
+        # non-overlapping patches -> rows (a pure permutation), zero-padded to a multiple of 8 columns, fp16
+        patches = torch.zeros(B * npatch, P["kp"], dtype=torch.float16, device=dev)
+        patches[:, : Cc * p * p].copy_(x.reshape(B, Cc, gh, p, gw, p).permute(0, 2, 4, 1, 3, 5).reshape(B * npatch, Cc * p * p))
+        emb = torch.empty(B * npatch, D, dtype=torch.float16, device=dev)
+        ops.gemm(patches, P["patch_w"], emb, bias=P["patch_b"], residual=pos.repeat(B, 1))   # normalise + patch conv + position
+        tok = torch.empty(B, n, D, dtype=torch.float16, device=dev)
+        tok[:, 0].copy_(cls)
+        tok[:, 1:].copy_(emb.view(B, npatch, D))
+        h, _ = _run_layers(P["layers"], tok.view(B * n, D), B, n, c.num_attention_heads, 5, c.layer_norm_eps, causal=False)
+        y = torch.empty_like(h)
+        ops.layernorm(h, P["norm"][0], P["norm"][1], y, c.layer_norm_eps)
+        return y, B, n
+
+    @torch.no_grad()
+    def forward_features(self, x):
+        y, B, n = self.normed_tokens(x)
+        y = y.view(B, n, -1).float()
+        return {"x_norm_clstoken": y[:, 0], "x_norm_patchtokens": y[:, 1:]}
+
+
+class FrozenDinoV2Encoder(_Packable):
+    """ldm/modules/encoders/modules.py:279-315: ImageNet normalisation, DINOv2 ViT-g/14 (``model.*``, hub names; weights
+    through ``load_state_dict``), ``projector`` = Linear(1536, 1024) of cat(x_norm_clstoken, x_norm_patchtokens) -> fp32
+    [B, 1 + patches, 1024].  ``config``: a smaller ``Dinov2Model`` config, plus ``interpolate_offset`` and ``projection_dim``."""
+
+    def __init__(self, device="cuda", freeze=True, config=None):
+        super().__init__()
+        c = _cfg(config if config is not None else {}, interpolate_offset=0.1, projection_dim=1024)
+        self.model = Dinov2Model(config, c.interpolate_offset, IMAGENET_MEAN, IMAGENET_STD)
+        self.device = device
+        if freeze:
+            self.freeze()
+        self.projector = _Param((c.projection_dim, self.model.config.hidden_size))
+
+    def freeze(self):
+        self.model.eval()
+        for p in self.model.parameters():
+            p.requires_grad = False
+
+    def _build_pack(self, dev):
+        return {"w": _h(self.projector.weight, dev), "b": _f(self.projector.bias, dev)}
+
+    @torch.no_grad()
+    def forward(self, image):
+        if isinstance(image, list):
+            image = torch.cat(image, 0)
+        P = self._packed()
+        y, B, n = self.model.normed_tokens(image)
+        out = torch.empty(B * n, P["w"].shape[0], dtype=torch.float32, device=y.device)
+        ops.gemm(y, P["w"], out, bias=P["b"])
+        return out.view(B, n, -1)
+
+    def encode(self, image):
+        return self(image)
 
 
 # ---- IP-Adapter projectors ---------------------------------------------------------------------------------------------------

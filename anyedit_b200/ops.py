@@ -248,12 +248,13 @@ def row_stats_buffer(M, C, device):
 
 
 def gemm(A, W, out, bias=None, rowadd=None, rows_per_batch=0, residual=None, act=0, M=None, K=None, lda=None,
-         N=None, ldw=None, ld_rowadd=None, stats_images=0, row_stats=None, ln=None):
+         N=None, ldw=None, ld_rowadd=None, stats_images=0, row_stats=None, ln=None, col_scale=None):
     """out[M, N'] = epilogue(A[M, K] @ W[N, K]^T); see anysd_gemm_params.
     ``stats_images`` > 0 (with ``rows_per_batch`` = rows of one image): also produce the GroupNorm statistics of ``out`` in the
     epilogue; returns a GnStats (None when the shape cannot).
     ``row_stats`` (row_stats_buffer(M, N)): per-row moments of ``out`` for a LayerNorm folded into the consumer.
-    ``ln`` = (row statistics of A, column sums of the gamma-scaled W, eps): LayerNorm(A) @ W^T + b with A un-normalised."""
+    ``ln`` = (row statistics of A, column sums of the gamma-scaled W, eps): LayerNorm(A) @ W^T + b with A un-normalised.
+    ``col_scale`` (fp32 [N]): out = residual + col_scale * (A @ W^T + bias), the LayerScale of a ViT block (act 0 only)."""
     _cuda(A, W, out)
     p = GemmParams()
     p.A, p.W, p.out = A.data_ptr(), W.data_ptr(), out.data_ptr()
@@ -280,6 +281,9 @@ def gemm(A, W, out, bias=None, rowadd=None, rows_per_batch=0, residual=None, act
         assert lst.dtype == torch.float32 and lst.is_contiguous() and lst.numel() == (p.K // 64) * p.M * 2, "ln statistics shape"
         assert lcs.dtype == torch.float32 and lcs.is_contiguous() and lcs.numel() == p.N and bias is not None
         p.ln_stats, p.ln_colsum, p.ln_eps = lst.data_ptr(), lcs.data_ptr(), float(leps)
+    if col_scale is not None:
+        assert col_scale.dtype == torch.float32 and col_scale.is_cuda and col_scale.is_contiguous() and col_scale.numel() == p.N
+        p.col_scale = col_scale.data_ptr()
     st = _want_stats(p, stats_images, out.device) if stats_images > 0 else None
     _sk = _want_splitk(p, out.device) if (row_stats is None and ln is None) else None
     with _Traced("gemm", 2.0 * p.M * p.N * p.K, f"M={p.M} N={p.N} K={p.K} act={p.act} res={int(residual is not None)}"):

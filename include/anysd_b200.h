@@ -110,7 +110,8 @@ int anysd_layernorm_f16(const void* x, const float* gamma, const float* beta, vo
  * out[m, n] = act(sum_k A[m,k] W[n,k] + bias[n] + rowadd[m / rows_per_batch, n]) + residual[m, n]
  * fp16 operands, fp32 accumulate.  act: 0 none, 1 SiLU, 2 GEGLU (W rows interleaved (a_j, gate_j);
  * out has N/2 columns: (acc_a + b_a) * gelu_erf(acc_g + b_g)), 3 GELU (erf; nn.GELU of the CLIP-H MLP and the Resampler
- * FeedForward), 4 QuickGELU (x sigmoid(1.702 x), the CLIP-L MLP). */
+ * FeedForward), 4 QuickGELU (x sigmoid(1.702 x), the CLIP-L MLP), 5 SwiGLU (layout of GEGLU, out = (acc_a + b_a) *
+ * silu(acc_g + b_g); the DINOv2 ViT-g/14 MLP; dense only, EUNSUPPORTED with conv). */
 typedef struct {
     const void* A;          /* dense: fp16 [M, lda]; conv: NHWC fp16 image [Nimg, H, W, Cin] */
     const void* W;          /* fp16 [N, ldw], row n = output channel, K contiguous ((ky,kx,ci) for conv) */
@@ -152,6 +153,9 @@ typedef struct {
                                W[n,k] gamma[k], bias[n] = b[n] + sum_k beta[k] W[n,k] (required) and */
     const float* ln_colsum; /* fp32 [N]: sum_k of the fp16 values of the packed W row n (16-byte aligned) */
     float ln_eps;
+    const float* col_scale; /* optional fp32 [N]: per-column output scale (LayerScale of a ViT block):
+                               out = residual + col_scale[n] (acc + bias[n] + rowadd), one fp16 rounding at the end.  Only with
+                               act 0, dense, no stats / row_stats / ln_stats (EUNSUPPORTED otherwise); never split-K.  NULL: off. */
 } anysd_gemm_params;
 int anysd_gemm_f16(const anysd_gemm_params* p, anysd_stream_t stream);
 /* Slabs per image of the statistics layout for this contraction, or 0 when the shape cannot produce them (rows of one
