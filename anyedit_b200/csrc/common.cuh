@@ -30,9 +30,9 @@ __device__ __forceinline__ float silu_f(float v) { return v / (1.0f + __expf(-v)
 __device__ __forceinline__ float gelu_erf_f(float v) { return 0.5f * v * (1.0f + erff(v * 0.70710678118654752440f)); }
 // QuickGELU of the OpenAI CLIP towers (transformers activations.py: x * sigmoid(1.702 x))
 __device__ __forceinline__ float quick_gelu_f(float v) { return v / (1.0f + __expf(-1.702f * v)); }
-// epilogue activations of anysd_gemm_params::act other than GEGLU: 1 SiLU, 3 GELU (erf), 4 QuickGELU
+// epilogue activations of anysd_gemm_params::act other than GEGLU: 1 SiLU, 3 GELU (erf), 4 QuickGELU, 6 ReLU
 __device__ __forceinline__ float act_f(float v, int act) {
-    return act == 1 ? silu_f(v) : (act == 3 ? gelu_erf_f(v) : (act == 4 ? quick_gelu_f(v) : v));
+    return act == 1 ? silu_f(v) : (act == 3 ? gelu_erf_f(v) : (act == 4 ? quick_gelu_f(v) : (act == 6 ? fmaxf(v, 0.0f) : v)));
 }
 
 __device__ __forceinline__ float warp_sum(float v) {

@@ -22,7 +22,7 @@ extern "C" int anysd_gemm_f16(const anysd_gemm_params* p, anysd_stream_t stream)
                   "gemm: K=%d and ldw=%d must be multiples of 8 with ldw >= K", p->K, p->ldw);
     ANYSD_REQUIRE(((uintptr_t)p->A % 16) == 0 && ((uintptr_t)p->W % 16) == 0, ANYSD_EINVAL,
                   "gemm: A and W must be 16-byte aligned");
-    ANYSD_REQUIRE(p->act >= 0 && p->act <= 5, ANYSD_EINVAL, "gemm: bad act %d", p->act);
+    ANYSD_REQUIRE(p->act >= 0 && p->act <= 6, ANYSD_EINVAL, "gemm: bad act %d", p->act);
     ANYSD_REQUIRE(p->out_dtype == ANYSD_F16 || p->out_dtype == ANYSD_F32, ANYSD_EINVAL, "gemm: bad out dtype");
     const bool glu = p->act == 2 || p->act == 5;
     const int n_out = glu ? p->N / 2 : p->N;

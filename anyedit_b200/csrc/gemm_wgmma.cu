@@ -7,7 +7,7 @@
 //     map's out-of-bounds fill), a ring of STAGES x (16 KB A + BN x 128 B of B), 128-byte swizzle;
 //   * warpgroups 1 and 2: 64 rows of the tile each, wgmma m64nBNk16 into register accumulators while the producer
 //     already streams the next unit's operands; the epilogue works on the accumulator fragment in place: bias or
-//     folded LayerNorm, time-embedding row add, per-column scale (LayerScale), SiLU / GELU / QuickGELU / GEGLU / SwiGLU,
+//     folded LayerNorm, time-embedding row add, per-column scale (LayerScale), SiLU / GELU / QuickGELU / ReLU / GEGLU / SwiGLU,
 //     residual, fp16 or fp32 stores, GroupNorm statistics (per 32-row slab and channel) and LayerNorm row statistics (per
 //     64-column slab) of the output.
 #include <cuda.h>
@@ -437,6 +437,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 #pragma unroll
                     for (int e = 0; e < 2; ++e)
                         v[h][e] = p.act == 1 ? silu_f(v[h][e])
+                                : p.act == 6 ? fmaxf(v[h][e], 0.0f)
                                              : (p.act == 3 ? (p.out_f16 ? p_gelu(v[h][e]) : gelu_erf_f(v[h][e])) : quick_gelu_f(v[h][e]));
             }
 #pragma unroll

@@ -394,9 +394,10 @@ class _LayerScale(nn.Module):
 
 
 class _DinoBlock(nn.Module):
-    """Hub ``NestedTensorBlock`` parameter holder: norm1, attn.{qkv, proj}, ls1, norm2, mlp.{w12, w3} (SwiGLUFFNFused), ls2."""
+    """Hub ``NestedTensorBlock`` parameter holder: norm1, attn.{qkv, proj}, ls1, norm2, mlp, ls2; the MLP is
+    ``mlp.{w12, w3}`` (SwiGLUFFNFused) or ``mlp.{fc1, fc2}`` (the GELU ``Mlp``)."""
 
-    def __init__(self, d, hidden):
+    def __init__(self, d, hidden, swiglu=True):
         super().__init__()
         self.norm1 = _Param((d,), kind="norm")
         self.attn = nn.Module()
@@ -404,25 +405,42 @@ class _DinoBlock(nn.Module):
         self.ls1 = _LayerScale(d)
         self.norm2 = _Param((d,), kind="norm")
         self.mlp = nn.Module()
-        self.mlp.w12, self.mlp.w3 = _Param((2 * hidden, d)), _Param((d, hidden))
+        if swiglu:
+            self.mlp.w12, self.mlp.w3 = _Param((2 * hidden, d)), _Param((d, hidden))
+        else:
+            self.mlp.fc1, self.mlp.fc2 = _Param((hidden, d)), _Param((d, hidden))
         self.ls2 = _LayerScale(d)
 
 
+# ``depth_anything_v2/dinov2.py`` ``DINOv2(model_name)``: patch 14, a 518 x 518 position table, LayerScale, offset 0.1
+DINOV2_CONFIGS = {
+    "vits": dict(hidden_size=384, num_attention_heads=6, num_hidden_layers=12, use_swiglu_ffn=False),
+    "vitb": dict(hidden_size=768, num_attention_heads=12, num_hidden_layers=12, use_swiglu_ffn=False),
+    "vitl": dict(hidden_size=1024, num_attention_heads=16, num_hidden_layers=24, use_swiglu_ffn=False),
+    "vitg": dict(hidden_size=1536, num_attention_heads=24, num_hidden_layers=40, use_swiglu_ffn=True),
+}
+
+
 class Dinov2Model(_Packable):
-    """DINOv2 ``DinoVisionTransformer`` with the SwiGLU MLP (hub ``dinov2_vitg14``) under the hub's parameter names.
+    """DINOv2 ``DinoVisionTransformer`` under the hub's parameter names, with the SwiGLU MLP (hub ``dinov2_vitg14``) or the GELU
+    ``Mlp`` (``use_swiglu_ffn=False``: ViT-S/B/L, exact-erf GELU in the fc1 epilogue).
     ``config``: dict or transformers ``Dinov2Config`` (hidden_size, num_hidden_layers, num_attention_heads, mlp_ratio, image_size
-    = the resolution of the position table, patch_size, layer_norm_eps); the defaults are ViT-g/14.  ``interpolate_offset``:
-    see ``dinov2_pos_table``.  ``pixel_mean`` / ``pixel_std`` (per channel): an input normalisation folded into the packed
-    patch embedding.  ``forward_features(x)`` -> {"x_norm_clstoken": [B, D], "x_norm_patchtokens": [B, gh*gw, D]} fp32."""
+    = the resolution of the position table, patch_size, layer_norm_eps, use_swiglu_ffn); the defaults are ViT-g/14; the
+    configurations of ``DINOv2(model_name)`` are ``DINOV2_CONFIGS``.  ``interpolate_offset``: see ``dinov2_pos_table``.
+    ``pixel_mean`` / ``pixel_std`` (per channel): an input normalisation folded into the packed patch embedding.
+    ``forward_features(x)`` -> {"x_norm_clstoken": [B, D], "x_norm_patchtokens": [B, gh*gw, D]} fp32;
+    ``get_intermediate_layers`` as the hub's."""
 
     def __init__(self, config=None, interpolate_offset=0.1, pixel_mean=None, pixel_std=None):
         super().__init__()
         self.config = c = _cfg(config if config is not None else {}, hidden_size=1536, num_hidden_layers=40, num_attention_heads=24,
                                mlp_ratio=4, image_size=518, patch_size=14, num_channels=3, layer_norm_eps=1e-6, use_swiglu_ffn=True)
-        if not c.use_swiglu_ffn:
-            raise NotImplementedError("Dinov2Model: only the SwiGLU MLP of ViT-g/14 is implemented")
         D, p = c.hidden_size, c.patch_size
-        hidden = (int(int(D * c.mlp_ratio) * 2 / 3) + 7) // 8 * 8     # SwiGLUFFNFused: 6144 -> 4096 for ViT-g
+        if c.use_swiglu_ffn:
+            hidden = (int(int(D * c.mlp_ratio) * 2 / 3) + 7) // 8 * 8     # SwiGLUFFNFused: 6144 -> 4096 for ViT-g
+        else:
+            hidden = int(D * c.mlp_ratio)
+        self._act = 5 if c.use_swiglu_ffn else 3
         m = c.image_size // p
         self.interpolate_offset, self.pixel_mean, self.pixel_std = interpolate_offset, pixel_mean, pixel_std
         self.cls_token = nn.Parameter(torch.zeros(1, 1, D))
@@ -430,7 +448,7 @@ class Dinov2Model(_Packable):
         self.mask_token = nn.Parameter(torch.zeros(1, D))           # masked pre-training only; loaded, never used
         self.patch_embed = nn.Module()
         self.patch_embed.proj = _Param((D, c.num_channels, p, p), kind="conv")
-        self.blocks = nn.ModuleList([_DinoBlock(D, hidden) for _ in range(c.num_hidden_layers)])
+        self.blocks = nn.ModuleList([_DinoBlock(D, hidden, c.use_swiglu_ffn) for _ in range(c.num_hidden_layers)])
         self.norm = _Param((D,), kind="norm")
 
     def _build_pack(self, dev):
@@ -448,15 +466,19 @@ class Dinov2Model(_Packable):
         wp[:, :k] = w.reshape(D, k)
         layers = []
         for L in self.blocks:
-            w12, b12 = L.mlp.w12.weight, L.mlp.w12.bias
-            hd = w12.shape[0] // 2
-            # act 5 takes rows (a_j, gate_j); the hub computes silu(x1) * x2 with x1, x2 = w12(x).chunk(2): a = x2, gate = x1
-            perm = torch.stack([torch.arange(hd, 2 * hd), torch.arange(hd)], 1).reshape(-1).to(w12.device)
+            if self._act == 5:
+                w12, b12 = L.mlp.w12.weight, L.mlp.w12.bias
+                hd = w12.shape[0] // 2
+                # act 5 takes rows (a_j, gate_j); the hub computes silu(x1) * x2 with x1, x2 = w12(x).chunk(2): a = x2, gate = x1
+                perm = torch.stack([torch.arange(hd, 2 * hd), torch.arange(hd)], 1).reshape(-1).to(w12.device)
+                fc1_w, fc1_b, fc2 = w12[perm], b12[perm], L.mlp.w3
+            else:
+                fc1_w, fc1_b, fc2 = L.mlp.fc1.weight, L.mlp.fc1.bias, L.mlp.fc2
             layers.append({"ln1": (_f(L.norm1.weight, dev), _f(L.norm1.bias, dev)), "ln2": (_f(L.norm2.weight, dev), _f(L.norm2.bias, dev)),
                            "qkv_w": _h(L.attn.qkv.weight, dev), "qkv_b": _f(L.attn.qkv.bias, dev),
                            "o_w": _h(L.attn.proj.weight, dev), "o_b": _f(L.attn.proj.bias, dev), "ls1": _f(L.ls1.gamma, dev),
-                           "fc1_w": _h(w12[perm], dev), "fc1_b": _f(b12[perm], dev),
-                           "fc2_w": _h(L.mlp.w3.weight, dev), "fc2_b": _f(L.mlp.w3.bias, dev), "ls2": _f(L.ls2.gamma, dev)})
+                           "fc1_w": _h(fc1_w, dev), "fc1_b": _f(fc1_b, dev),
+                           "fc2_w": _h(fc2.weight, dev), "fc2_b": _f(fc2.bias, dev), "ls2": _f(L.ls2.gamma, dev)})
         return {"patch_w": _h(wp, dev), "patch_b": _f(b, dev), "kp": kp, "layers": layers,
                 "norm": (_f(self.norm.weight, dev), _f(self.norm.bias, dev)), "pos": {}}
 
@@ -469,8 +491,8 @@ class Dinov2Model(_Packable):
             P["pos"][(gh, gw)] = (cls.half().contiguous(), t[1:].half().contiguous())
         return P["pos"][(gh, gw)]
 
-    def normed_tokens(self, x):
-        """-> (fp16 [B * (1 + gh*gw), D] = the final LayerNorm of every token, class token first per image; B; 1 + gh*gw)."""
+    def _tokens(self, x):
+        """-> (fp16 [B * (1 + gh*gw), D] = class token + patch embeddings + positions, class token first per image; B; gh; gw)."""
         P, c = self._packed(), self.config
         dev = P["patch_w"].device
         x = x.to(dev)
@@ -488,10 +510,64 @@ class Dinov2Model(_Packable):
         tok = torch.empty(B, n, D, dtype=torch.float16, device=dev)
         tok[:, 0].copy_(cls)
         tok[:, 1:].copy_(emb.view(B, npatch, D))
-        h, _ = _run_layers(P["layers"], tok.view(B * n, D), B, n, c.num_attention_heads, 5, c.layer_norm_eps, causal=False)
+        return tok.view(B * n, D), B, gh, gw
+
+    def normed_tokens(self, x):
+        """-> (fp16 [B * (1 + gh*gw), D] = the final LayerNorm of every token, class token first per image; B; 1 + gh*gw)."""
+        P, c = self._packed(), self.config
+        tok, B, gh, gw = self._tokens(x)
+        n = gh * gw + 1
+        h, _ = _run_layers(P["layers"], tok, B, n, c.num_attention_heads, self._act, c.layer_norm_eps, causal=False)
         y = torch.empty_like(h)
         ops.layernorm(h, P["norm"][0], P["norm"][1], y, c.layer_norm_eps)
         return y, B, n
+
+    def _block_outputs(self, x, blocks):
+        """Run the blocks up to the last of ``blocks`` (indices into self.blocks) -> ([fp16 [B * n, D] output of each requested
+        block], B, gh, gw)."""
+        P, c = self._packed(), self.config
+        blocks = [b % len(P["layers"]) for b in blocks]
+        tok, B, gh, gw = self._tokens(x)
+        _, hidden = _run_layers(P["layers"], tok, B, gh * gw + 1, c.num_attention_heads, self._act, c.layer_norm_eps, causal=False,
+                                keep_hidden=True, n_run=max(blocks) + 1)
+        return [hidden[b + 1] for b in blocks], B, gh, gw
+
+    def intermediate_patches(self, x, blocks):
+        """The depth head's input: for each block in ``blocks``, the final LayerNorm of its output on the PATCH rows only, densely
+        packed fp16 [B * gh * gw, D] (an image's patch rows are contiguous, so each image is normalised straight into the buffer).
+        -> (list, B, gh, gw)."""
+        P, c = self._packed(), self.config
+        outs, B, gh, gw = self._block_outputs(x, blocks)
+        n, D = gh * gw + 1, c.hidden_size
+        res = []
+        for h in outs:
+            y = torch.empty(B, n - 1, D, dtype=torch.float16, device=h.device)
+            for b in range(B):
+                ops.layernorm(h.view(B, n, D)[b, 1:], P["norm"][0], P["norm"][1], y[b], c.layer_norm_eps)
+            res.append(y.view(B * (n - 1), D))
+        return res, B, gh, gw
+
+    @torch.no_grad()
+    def get_intermediate_layers(self, x, n=1, reshape=False, return_class_token=False, norm=True):
+        """``DinoVisionTransformer.get_intermediate_layers`` (depth_anything_v2/dinov2.py:271-321): ``n`` = the number of last
+        blocks or a list of block indices; the blocks run only up to the last one requested.  fp32 outputs [B, gh*gw, D]
+        ([B, D, gh, gw] with ``reshape``), paired with the class tokens [B, D] when ``return_class_token``."""
+        L = len(self.blocks)
+        blocks = list(range(L - n, L)) if isinstance(n, int) else list(n)
+        outs, B, gh, gw = self._block_outputs(x, blocks)
+        P, c = self._packed(), self.config
+        res = []
+        for h in outs:
+            if norm:
+                y = torch.empty_like(h)
+                ops.layernorm(h, P["norm"][0], P["norm"][1], y, c.layer_norm_eps)
+                h = y
+            res.append(h.view(B, gh * gw + 1, -1).float())
+        cls = [t[:, 0] for t in res]
+        res = [t[:, 1:] for t in res]
+        if reshape:
+            res = [t.reshape(B, gh, gw, -1).permute(0, 3, 1, 2).contiguous() for t in res]
+        return tuple(zip(res, cls)) if return_class_token else tuple(res)
 
     @torch.no_grad()
     def forward_features(self, x):

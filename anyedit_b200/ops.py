@@ -447,6 +447,45 @@ def attention_small(q, k, v, out, B, heads, n_q, n_kv, d, ld_q, ld_k, ld_v, ld_o
     _count()
 
 
+# ---- dense prediction (the Depth Anything V2 DPT head) -------------------------------------------------------------
+def resize_bilinear(x, y, addend=None):
+    """F.interpolate(mode="bilinear", align_corners=True): x NHWC fp16 [N, H, W, C] -> y [N, Ho, Wo, C] (C % 8 == 0), with
+    ``addend`` (fp16, y's shape) added before the rounding; or fp32 single-channel maps x [N, H, W] -> y [N, Ho, Wo]."""
+    _cuda(x, y, addend)
+    assert x.is_contiguous() and y.is_contiguous() and x.dtype == y.dtype
+    if x.dtype == torch.float32:
+        assert x.dim() == 3 and y.dim() == 3 and addend is None and x.shape[0] == y.shape[0]
+        N, H, W = x.shape
+        _lib.check(_lib.load().anysd_resize_bilinear_ac_f32(_ptr(x), _ptr(y), N, H, W, y.shape[1], y.shape[2], _stream()),
+                   "resize_bilinear")
+    else:
+        N, H, W, Cc = x.shape
+        assert x.dtype == torch.float16 and y.shape[0] == N and y.shape[3] == Cc
+        if addend is not None:
+            assert addend.shape == y.shape and addend.dtype == torch.float16 and addend.is_contiguous()
+        _lib.check(_lib.load().anysd_resize_bilinear_ac_f16(_ptr(x), _ptr(addend), _ptr(y), N, H, W, Cc, y.shape[1], y.shape[2],
+                                                            _stream()), "resize_bilinear")
+    _count()
+
+
+def relu(x, y):
+    """y = max(x, 0), fp16, into a separate buffer."""
+    _cuda(x, y)
+    assert x.dtype == y.dtype == torch.float16 and x.is_contiguous() and y.is_contiguous() and x.numel() == y.numel()
+    _lib.check(_lib.load().anysd_relu_f16(_ptr(x), _ptr(y), x.numel(), _stream()), "relu")
+    _count()
+
+
+def depth_to_space(g, out, r):
+    """g fp16 [B*gh*gw, r*r*C] with columns (ky, kx, c) -> out NHWC fp16 [B, r*gh, r*gw, C]."""
+    _cuda(g, out)
+    B, Ho, Wo, Cc = out.shape
+    assert g.is_contiguous() and out.is_contiguous() and g.dtype == out.dtype == torch.float16
+    assert Ho % r == 0 and Wo % r == 0 and tuple(g.shape) == (B * (Ho // r) * (Wo // r), r * r * Cc)
+    _lib.check(_lib.load().anysd_depth_to_space_f16(_ptr(g), _ptr(out), B, Ho // r, Wo // r, r, Cc, _stream()), "depth_to_space")
+    _count()
+
+
 # ---- training step (SURVEY.md a24): thin wrappers, same conventions as above -------------------------------------
 def q_sample(x0, noise, t, sqrt_acp, sqrt_1m_acp, out):
     _cuda(x0, noise, t, out)

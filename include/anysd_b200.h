@@ -111,7 +111,8 @@ int anysd_layernorm_f16(const void* x, const float* gamma, const float* beta, vo
  * fp16 operands, fp32 accumulate.  act: 0 none, 1 SiLU, 2 GEGLU (W rows interleaved (a_j, gate_j);
  * out has N/2 columns: (acc_a + b_a) * gelu_erf(acc_g + b_g)), 3 GELU (erf; nn.GELU of the CLIP-H MLP and the Resampler
  * FeedForward), 4 QuickGELU (x sigmoid(1.702 x), the CLIP-L MLP), 5 SwiGLU (layout of GEGLU, out = (acc_a + b_a) *
- * silu(acc_g + b_g); the DINOv2 ViT-g/14 MLP; dense only, EUNSUPPORTED with conv). */
+ * silu(acc_g + b_g); the DINOv2 ViT-g/14 MLP; dense only, EUNSUPPORTED with conv), 6 ReLU (max(x, 0); the Depth Anything
+ * DPT head, dense and conv). */
 typedef struct {
     const void* A;          /* dense: fp16 [M, lda]; conv: NHWC fp16 image [Nimg, H, W, Cin] */
     const void* W;          /* fp16 [N, ldw], row n = output channel, K contiguous ((ky,kx,ci) for conv) */
@@ -253,6 +254,22 @@ int anysd_embed_tokens_f16(const long long* ids, const void* tok_table, const vo
  * at columns [h d, (h+1) d), same for k, v ([B*n_kv, ld_k|ld_v]) and out; causal != 0: key j masked for query i when j > i. */
 int anysd_attention_small_f16(const void* q, const void* k, const void* v, void* out, int B, int heads, int n_q, int n_kv, int d,
                               int ld_q, int ld_k, int ld_v, int ld_o, float scale, int causal, anysd_stream_t stream);
+
+/* ==== dense prediction: the Depth Anything V2 DPT head (AnyEdit_Collection/other_modules/depth_anything_v2/dpt.py,
+ * util/blocks.py); its 1x1 / 3x3 convolutions and projections run on anysd_gemm_f16 ========================================
+ * F.interpolate(x, (Ho, Wo), mode="bilinear", align_corners=True) on NHWC fp16 [N, H, W, C] -> y [N, Ho, Wo, C], any sizes,
+ * C % 8 == 0; src = dst (in - 1) / (out - 1) in fp32 as ATen computes it.  addend (fp16 [N, Ho, Wo, C]) or NULL: added in fp32
+ * before the one rounding (the FeatureFusionBlock sum `path + layer_rn`, blocks.py:132-134). */
+int anysd_resize_bilinear_ac_f16(const void* x, const void* addend, void* y, int N, int H, int W, int C, int Ho, int Wo,
+                                 anysd_stream_t stream);
+/* the same on fp32 single-channel maps [N, H, W] -> [N, Ho, Wo] (DepthAnythingV2.infer_image, dpt.py:192) */
+int anysd_resize_bilinear_ac_f32(const float* x, float* y, int N, int H, int W, int Ho, int Wo, anysd_stream_t stream);
+/* y = max(x, 0) into a separate buffer (ResidualConvUnit, blocks.py:70-71: x stays the residual); fp16, n % 8 == 0 */
+int anysd_relu_f16(const void* x, void* y, long long n, anysd_stream_t stream);
+/* ConvTranspose2d(kernel = stride = r, padding 0) (dpt.py:63-74) = one contraction of the patch rows with the weight packed
+ * [(ky, kx, co), ci] (bias repeated r^2 times) giving g [B gh gw, r r C], then this re-layout:
+ * out[b, y r + ky, x r + kx, c] = g[(b gh + y) gw + x, (ky r + kx) C + c]; fp16, C % 8 == 0. */
+int anysd_depth_to_space_f16(const void* g, void* out, int B, int gh, int gw, int r, int C, anysd_stream_t stream);
 
 /* ==== training step (SURVEY.md a24; train.py:629-710) =====================================================
  * The reference back-propagates mse_loss(MoE(...), noise) through the frozen UNet with torch autograd
