@@ -5,13 +5,18 @@
 //     n-tile fastest so that the CTAs running concurrently share A rows and weight tiles in L2;
 //   * warp 0: TMA producer (2-D map for token matrices, 4-D NHWC map for conv patches: the conv's zero padding is the
 //     map's out-of-bounds fill), a ring of STAGES x (16 KB A + BN x 128 B of B), 128-byte swizzle;
-//   * warpgroups 1 and 2: 64 rows of the tile each, wgmma m64nBNk16 into register accumulators while the producer
-//     already streams the next unit's operands; the epilogue works on the accumulator fragment in place: bias or
+//   * warpgroups 1 and 2, cooperative schedule: 64 rows of the tile each, wgmma m64nBNk16 into register accumulators while
+//     the producer already streams the next unit's operands;
+//   * warpgroups 1 and 2, ping-pong schedule (BN 64 / 128, no split-K): each owns whole units -- the CTA's i-th unit goes to
+//     warpgroup i & 1 -- and issues its mainloop only while it holds the tensor-core turn, which it passes on as soon as its
+//     last product is issued, so that its epilogue runs under the other warpgroup's products;
+//   * the epilogue works on the accumulator fragment in place: bias or
 //     folded LayerNorm, time-embedding row add, per-column scale (LayerScale), SiLU / GELU / QuickGELU / ReLU / GEGLU / SwiGLU,
 //     residual, fp16 or fp32 stores, GroupNorm statistics (per 32-row slab and channel) and LayerNorm row statistics (per
 //     64-column slab) of the output.
 #include <cuda.h>
 #include <stdlib.h>
+#include <string.h>
 
 #include "common.cuh"
 #include "wgmma.cuh"
@@ -96,6 +101,10 @@ __device__ __forceinline__ void g_tma_4d(uint32_t dst, const CUtensorMap* tm, ui
 // named barrier of the two warps that share a 32-row slab (ids 1..4), of one consumer warpgroup (ids 5, 6)
 __device__ __forceinline__ void g_pair_bar(int id) { asm volatile("bar.sync %0, 64;" ::"r"(id) : "memory"); }
 __device__ __forceinline__ void g_wg_bar(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
+// ping-pong turns: consumer warpgroup c waits on named barrier 7 + c before it issues a unit's products, and then arrives on
+// the other one's (both count the 256 consumer threads)
+__device__ __forceinline__ void g_turn_wait(int c) { asm volatile("bar.sync %0, 256;" ::"r"(7 + c) : "memory"); }
+__device__ __forceinline__ void g_turn_pass(int c) { asm volatile("bar.arrive %0, 256;" ::"r"(8 - c) : "memory"); }
 
 // Exact (erf) GELU  x Phi(x)  in 11 instructions: Phi(x) = 1 / (1 + 2^(-x P(x^2))) with a cubic P fitted (minimax on the ABSOLUTE
 // error of x Phi(x), x^2 clamped at 36 -- beyond it the logistic is saturated either way) to |err| < 1.2e-5 for all x: 1/40 of the
@@ -133,9 +142,10 @@ __device__ __forceinline__ TileCoord tile_coord(const GArgs& p, int tile) {
     return c;
 }
 
-template <int BN, bool CONV>
+template <int BN, bool CONV, bool PP>
 __global__ void __launch_bounds__(G_THREADS, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GArgs p) {
+    static_assert(!PP || BN <= 128, "ping-pong: a whole 128 x BN tile per warpgroup, at most 128 accumulators per thread");
     using Cfg = GCfg<BN>;
     constexpr int STAGES = Cfg::STAGES;
     extern __shared__ unsigned char g_smem_raw[];
@@ -155,7 +165,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
         for (int s = 0; s < STAGES; ++s) {
             g_bar_init(full_bar(s), 1);
-            g_bar_init(empty_bar(s), 8);      // one arrive per consumer warp
+            g_bar_init(empty_bar(s), PP ? 4 : 8);   // one arrive per consumer warp that reads the stage
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
@@ -195,11 +205,9 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 
     // ===== consumer warpgroups =====
     asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
-    const int wg = (warp >> 2) - 1;                       // rows 64 wg .. 64 wg + 63 of the tile
-    const int wq = warp & 3;                              // rows 16 wq .. of the warpgroup's 64
-    const int ew = wg * 4 + wq;                           // consumer warp 0..7
-    const int slab = ew >> 1;                             // 32-row slab of the tile (two warps)
-    const int rl0 = wg * 64 + wq * 16 + (lane >> 2);      // this thread's tile rows: rl0, rl0 + 8
+    const int wg = (warp >> 2) - 1;                       // cooperative: rows 64 wg .. 64 wg + 63 of the tile
+    const int wq = warp & 3;                              // rows 16 wq .. of a 64-row half
+    const int ew = wg * 4 + wq;                           // consumer warp 0..7; warps ew, ew ^ 1 share a 32-row slab
     const int q4 = lane & 3;
     const bool ln_in = !CONV && p.ln_stats != nullptr;
     const bool row_st = !CONV && p.row_stats != nullptr;
@@ -213,9 +221,13 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     float* s_cs = s_bias + BN;
     const float* colv = ln_in ? p.ln_colsum : (col_sc ? p.col_scale : nullptr);   // what s_cs holds (never both)
     const int wtid = threadIdx.x & 127;
-    float acc[BN / 2];
+    // ping-pong: the whole tile, rows 0..63 in acc[0, BN / 2), rows 64..127 in acc[BN / 2, BN)
+    float acc[PP ? BN : BN / 2];
     uint32_t g = 0;
-    for (int unit = blockIdx.x; unit < p.num_units; unit += gridDim.x) {
+    const int ustep = PP ? 2 * gridDim.x : gridDim.x;
+    for (int unit = blockIdx.x + (PP ? wg * gridDim.x : 0); unit < p.num_units; unit += ustep) {
+        // ping-pong never splits K: the CTA's i-th unit fills ring slots i num_kb .. (i + 1) num_kb - 1
+        if (PP) g = (uint32_t)((unit - blockIdx.x) / gridDim.x) * p.num_kb;
         const int tile = unit / p.splits;
         const int kb0 = (unit - tile * p.splits) * p.kb_per_split;
         const int kb1 = kb0 + p.kb_per_split < p.num_kb ? kb0 + p.kb_per_split : p.num_kb;
@@ -229,14 +241,22 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             pc[r] = (j < BN && col < p.N && colv != nullptr) ? __ldg(colv + col) : 0.f;
         }
 #pragma unroll
-        for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+        for (int i = 0; i < (PP ? BN : BN / 2); ++i) acc[i] = 0.f;
+        // ping-pong turns: warpgroup 0 takes the CTA's first unit without waiting, and no turn is passed after the CTA's last
+        // unit, so every bar.sync meets exactly one bar.arrive.  The turn also keeps the two warpgroups' ring slots in ring
+        // order: a warpgroup starts waiting on its unit's stages only once every earlier stage has landed.
+        if (PP && unit >= (int)(blockIdx.x + gridDim.x)) g_turn_wait(wg);
         for (int kb = kb0; kb < kb1; ++kb, ++g) {
             const int s = g % STAGES;
             g_wait(full_bar(s), (g / STAGES) & 1);
-            const uint32_t sa = base + s * Cfg::STAGE_BYTES + wg * 64 * 128, sb = base + s * Cfg::STAGE_BYTES + G_A_BYTES;
+            const uint32_t sa = base + s * Cfg::STAGE_BYTES + (PP ? 0 : wg * 64 * 128), sb = base + s * Cfg::STAGE_BYTES + G_A_BYTES;
             wg_fence();
 #pragma unroll
-            for (int k = 0; k < G_BK / 16; ++k) Wgmma<BN>::ss(acc, wg_desc(sa + 32 * k, 16, 1024), wg_desc(sb + 32 * k, 16, 1024), 1);
+            for (int k = 0; k < G_BK / 16; ++k) {
+                Wgmma<BN>::ss(acc, wg_desc(sa + 32 * k, 16, 1024), wg_desc(sb + 32 * k, 16, 1024), 1);
+                if constexpr (PP)
+                    Wgmma<BN>::ss(acc + BN / 2, wg_desc(sa + 64 * 128 + 32 * k, 16, 1024), wg_desc(sb + 32 * k, 16, 1024), 1);
+            }
             wg_commit();
             wg_wait<1>();                                 // the previous k-block's products have read their stage
             if (kb > kb0) {
@@ -244,9 +264,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                 if (lane == 0) g_arrive(empty_bar((g - 1) % STAGES));
             }
         }
+        if (PP && unit + (int)gridDim.x < p.num_units) g_turn_pass(wg);
         wg_wait<0>();
 #pragma unroll
-        for (int i = 0; i < BN / 2; ++i) wg_fence_regs(acc[i]);
+        for (int i = 0; i < (PP ? BN : BN / 2); ++i) wg_fence_regs(acc[i]);
         if (kb1 > kb0) {
             __syncwarp();
             if (lane == 0) g_arrive(empty_bar((g - 1) % STAGES));
@@ -261,8 +282,18 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         }
         g_wg_bar(5 + wg);
 
+        // The epilogue runs once per 64-row half the warpgroup holds: its own half in the cooperative schedule, both halves of
+        // the unit in turn in the ping-pong one (unrolled, so that each pass reads its accumulators at static indices).
+        // Split-K is cooperative only, where this loop makes one pass: its `continue` leaves the unit.
+#pragma unroll
+        for (int hh = 0; hh < (PP ? 2 : 1); ++hh) {
+        const float* ea = acc + hh * (BN / 2);            // the pass's 64 rows in the fragment order of Wgmma<BN>
+        const int half = PP ? hh : wg;
+        const int slab = half * 2 + (wq >> 1);              // 32-row slab of the tile (warps ew, ew ^ 1)
+        const int rl0 = half * 64 + wq * 16 + (lane >> 2);  // this thread's tile rows: rl0, rl0 + 8
+
         // ---- split-K: dump this unit's raw accumulators; the slab's last unit adds all partials in split order ----
-        if (p.splits > 1) {
+        if (!PP && p.splits > 1) {
             const int ks = unit - tile * p.splits;
             const float* wst = p.sk_ws + (size_t)tile * p.splits * (G_BM * BN);
             float* mine = p.sk_ws + ((size_t)tile * p.splits + ks) * (G_BM * BN);
@@ -360,13 +391,13 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 #pragma unroll
             for (int u = 0; u < CH; ++u)
 #pragma unroll
-                for (int e = 0; e < 4; ++e) a[u][e] = acc[4 * u + e];
+                for (int e = 0; e < 4; ++e) a[u][e] = ea[4 * u + e];
 #pragma unroll
             for (int k = CH; k < BN / 8; k += CH)         // selects, not branches: no divergent accumulator access
 #pragma unroll
                 for (int u = 0; u < CH; ++u)
 #pragma unroll
-                    for (int e = 0; e < 4; ++e) a[u][e] = k == i0 ? acc[4 * (k + u) + e] : a[u][e];
+                    for (int e = 0; e < 4; ++e) a[u][e] = k == i0 ? ea[4 * (k + u) + e] : a[u][e];
             float2 ra[CH][2];                             // row adds and residuals of the chunk, in flight at once
             __half2 rr[CH][2];
 #pragma unroll
@@ -490,7 +521,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         }
         }
         if (p.stats != nullptr) {
-            g_pair_bar(1 + slab);
+            g_pair_bar(1 + (ew >> 1));                    // = 1 + slab in the cooperative schedule
             if ((ew & 1) == 0) {
                 int simg, sii;
                 if (CONV) {
@@ -511,7 +542,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                     }
                 }
             }
-            g_pair_bar(1 + slab);                         // read before the next tile's statistics overwrite it
+            g_pair_bar(1 + (ew >> 1));                    // read before the next tile's statistics overwrite it
+        }
         }
     }
 }
@@ -699,12 +731,17 @@ static int p_geometry_splits(const anysd_gemm_params* q, int num_kb) {
 // most of the machine idle while every busy SM streams a full K operand pair through its L2 port; mid levels suffer from
 // wave quantisation.  The per-tile constant 270 is inherited from the project's earlier GPU and kernel and has not been re-fitted
 // for this kernel on the H100 (only the SM count is the H100's).  ANYSD_GEMM_BN forces a width.
-static void p_select(const anysd_gemm_params* q, int tiles_m, int num_kb, int* bn_out, int* splits_out) {
+//
+// Ping-pong (never split) runs 128 wide.  It is chosen, from measurements on the H100 (DESIGN.md §3.1), when 128 divides N, every
+// CTA gets at least 4 units -- with fewer, one warpgroup runs a whole tile alone and the schedule loses -- and either K is short
+// (dense, at most 20 k-blocks: the epilogue is comparable to the mainloop) or the cooperative width does not divide N (N = 640:
+// 5 x 128 against 3 x 256).  64-wide ping-pong tiles lost on most shapes measured; they run only when ANYSD_GEMM_BN forces 64.
+// ANYSD_GEMM_SCHED=coop|pingpong forces the schedule where it is possible.
+static int p_width(const anysd_gemm_params* q, int tiles_m, int num_kb, int sp) {
     static const char* force_bn = getenv("ANYSD_GEMM_BN");
-    const int sp = splits_out ? p_geometry_splits(q, num_kb) : 1;
+    static const int widths[4] = {256, 192, 128, 64};     // 192 balances N = 320 (192 + 128) and divides 960 / 1920
     int bn = 256;
     double best = -1;
-    static const int widths[4] = {256, 192, 128, 64};     // 192 balances N = 320 (192 + 128) and divides 960 / 1920
     for (int wi = 0; wi < 4; ++wi) {
         const int w = widths[wi];
         if (force_bn && atoi(force_bn) != w) continue;
@@ -714,8 +751,29 @@ static void p_select(const anysd_gemm_params* q, int tiles_m, int num_kb, int* b
         const double cost = (double)rounds * (w + 270) * ((double)cdiv(num_kb, sp) + (sp > 1 ? 8.0 : 0.0));
         if (best < 0 || cost < best) { best = cost; bn = w; }
     }
-    *bn_out = bn;
+    return bn;
+}
+
+static void p_select(const anysd_gemm_params* q, int tiles_m, int num_kb, int* bn_out, int* splits_out, bool* pp_out) {
+    static const char* force_bn = getenv("ANYSD_GEMM_BN");
+    static const char* force_sched = getenv("ANYSD_GEMM_SCHED");
+    const int sp = splits_out ? p_geometry_splits(q, num_kb) : 1;
+    const int bn_coop = p_width(q, tiles_m, num_kb, sp);
+    bool pp = false;
+    if (sp == 1 && (!force_bn || atoi(force_bn) <= 128)) {
+        if (force_sched) pp = strcmp(force_sched, "pingpong") == 0;
+        else if (q->N % 128 == 0 && (long)tiles_m * (q->N / 128) >= 4L * sm_count())
+            pp = (!q->conv && num_kb <= 20) || q->N % bn_coop != 0;
+        if (pp) {
+            *bn_out = force_bn && atoi(force_bn) == 64 ? 64 : 128;
+            if (splits_out) *splits_out = 1;
+            *pp_out = true;
+            return;
+        }
+    }
+    *bn_out = bn_coop;
     if (splits_out) *splits_out = sp;
+    *pp_out = false;
 }
 static size_t p_splitk_bytes(int tiles_m, int N, int bn, int splits) {
     if (splits <= 1) return 0;
@@ -737,8 +795,9 @@ static void p_tiles(const anysd_gemm_params* q, int* tiles_m, int* num_kb) {
 // scratch the caller should provide for this contraction to run split-K (0: the schedule does not split it)
 size_t wg_splitk_bytes(const anysd_gemm_params* q) {
     int tiles_m, num_kb, bn, splits;
+    bool pp;
     p_tiles(q, &tiles_m, &num_kb);
-    p_select(q, tiles_m, num_kb, &bn, &splits);
+    p_select(q, tiles_m, num_kb, &bn, &splits, &pp);
     return p_splitk_bytes(tiles_m, q->N, bn, splits);
 }
 
@@ -780,14 +839,14 @@ bool wg_supported(const anysd_gemm_params* q) {
     return p_get_encode() != nullptr;
 }
 
-template <int BN, bool CONV>
+template <int BN, bool CONV, bool PP>
 static int p_launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const GArgs& a, cudaStream_t st) {
     static bool done[64];
     int dev = 0;
     cudaGetDevice(&dev);
     dev &= 63;
     if (!done[dev]) {
-        cudaError_t e = cudaFuncSetAttribute(gemm_wgmma_kernel<BN, CONV>, cudaFuncAttributeMaxDynamicSharedMemorySize, GCfg<BN>::SMEM);
+        cudaError_t e = cudaFuncSetAttribute(gemm_wgmma_kernel<BN, CONV, PP>, cudaFuncAttributeMaxDynamicSharedMemorySize, GCfg<BN>::SMEM);
         if (e != cudaSuccess) {
             set_error("wgmma gemm: smem opt-in failed: %s", cudaGetErrorString(e));
             return ANYSD_ECUDA;
@@ -796,17 +855,18 @@ static int p_launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const GArgs&
     }
     int grid = sm_count();
     if (grid > a.num_units) grid = a.num_units;
-    gemm_wgmma_kernel<BN, CONV><<<grid, G_THREADS, GCfg<BN>::SMEM, st>>>(tmA, tmB, a);
+    gemm_wgmma_kernel<BN, CONV, PP><<<grid, G_THREADS, GCfg<BN>::SMEM, st>>>(tmA, tmB, a);
     return check_launch(CONV ? "conv3x3 (wgmma)" : "gemm (wgmma)");
 }
 
 template <bool CONV>
-static int p_launch_bn(int bn, const CUtensorMap& tmA, const CUtensorMap& tmB, const GArgs& a, cudaStream_t st) {
+static int p_launch_bn(int bn, bool pp, const CUtensorMap& tmA, const CUtensorMap& tmB, const GArgs& a, cudaStream_t st) {
+    if (pp) return bn == 128 ? p_launch<128, CONV, true>(tmA, tmB, a, st) : p_launch<64, CONV, true>(tmA, tmB, a, st);
     switch (bn) {
-        case 256: return p_launch<256, CONV>(tmA, tmB, a, st);
-        case 192: return p_launch<192, CONV>(tmA, tmB, a, st);
-        case 128: return p_launch<128, CONV>(tmA, tmB, a, st);
-        default: return p_launch<64, CONV>(tmA, tmB, a, st);
+        case 256: return p_launch<256, CONV, false>(tmA, tmB, a, st);
+        case 192: return p_launch<192, CONV, false>(tmA, tmB, a, st);
+        case 128: return p_launch<128, CONV, false>(tmA, tmB, a, st);
+        default: return p_launch<64, CONV, false>(tmA, tmB, a, st);
     }
 }
 
@@ -883,12 +943,13 @@ int launch_gemm_wg(const anysd_gemm_params* q, cudaStream_t st) {
         ok = ok && p_map_2d(&tmA, q->A, (uint64_t)q->K, (uint64_t)q->M, (uint64_t)q->lda, G_BK, G_BM);
     }
     int bn = 256, splits = 1;
-    p_select(q, a.tiles_m, a.num_kb, &bn, &splits);
+    bool pp = false;
+    p_select(q, a.tiles_m, a.num_kb, &bn, &splits, &pp);
     const size_t sk_need = p_splitk_bytes(a.tiles_m, q->N, bn, splits);
     if (splits > 1 && (q->splitk_workspace == nullptr || q->splitk_workspace_bytes < sk_need || q->splitk_counters == nullptr ||
                        (size_t)a.tiles_m * cdiv(q->N, bn) * 4 * sizeof(unsigned int) > q->splitk_counters_bytes)) {
         splits = 1;                                   // no scratch from the caller: the plain schedule
-        p_select(q, a.tiles_m, a.num_kb, &bn, nullptr);
+        p_select(q, a.tiles_m, a.num_kb, &bn, nullptr, &pp);
     }
     a.tiles_n = cdiv(q->N, bn);
     ok = ok && p_map_2d(&tmB, q->W, (uint64_t)q->K, (uint64_t)q->N, (uint64_t)q->ldw, G_BK, bn);
@@ -902,7 +963,7 @@ int launch_gemm_wg(const anysd_gemm_params* q, cudaStream_t st) {
     a.num_units = a.num_tiles * splits;
     a.sk_ws = (float*)q->splitk_workspace;
     a.sk_cnt = (unsigned int*)q->splitk_counters;
-    return q->conv ? p_launch_bn<true>(bn, tmA, tmB, a, st) : p_launch_bn<false>(bn, tmA, tmB, a, st);
+    return q->conv ? p_launch_bn<true>(bn, pp, tmA, tmB, a, st) : p_launch_bn<false>(bn, pp, tmA, tmB, a, st);
 }
 
 }  // namespace anysd
