@@ -101,11 +101,16 @@ SIGNATURES = {
     "anysd_gaussian_posterior_f32": (_I, [_VP, _VP, _VP, _VP, _F, _I, _LL, _VP]),
     "anysd_embed_tokens_f16": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, _I, _VP]),
     "anysd_attention_small_f16": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _I, _I, _I, _I, _F, _I, _VP]),
-    # ---- dense prediction (Depth Anything V2 head) ----
-    "anysd_resize_bilinear_ac_f16": (_I, [_VP, _VP, _VP, _I, _I, _I, _I, _I, _I, _VP]),
+    # ---- dense prediction (Depth Anything V2 head, UniFormer + UPerNet segmentor) ----
+    "anysd_resize_bilinear_f16": (_I, [_VP, _VP, _VP, _I, _I, _I, _I, _I, _I, _I, _I, _VP]),
     "anysd_resize_bilinear_ac_f32": (_I, [_VP, _VP, _I, _I, _I, _I, _I, _VP]),
     "anysd_relu_f16": (_I, [_VP, _VP, _LL, _VP]),
     "anysd_depth_to_space_f16": (_I, [_VP, _VP, _I, _I, _I, _I, _I, _VP]),
+    "anysd_space_to_depth_f16": (_I, [_VP, _VP, _I, _I, _I, _I, _I, _VP]),
+    "anysd_space_to_depth_u8": (_I, [_VP, _VP, _I, _I, _I, _I, _I, _VP]),
+    "anysd_dwconv_f16": (_I, [_VP, _VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _VP]),
+    "anysd_adaptive_avg_pool_f16": (_I, [_VP, _VP, _I, _I, _I, _I, _I, _I, _VP]),
+    "anysd_seg_labels_f32": (_I, [_VP, _I, _I, _I, _I, _I, _I, _I, _I, _I, _VP, _VP, _VP, _VP]),
     # ---- training step ----
     "anysd_q_sample_f32": (_I, [_VP, _VP, _VP, _VP, _VP, _VP, _I, _LL, _VP]),
     "anysd_mse_workspace_bytes": (_SZ, []),

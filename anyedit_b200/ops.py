@@ -447,24 +447,28 @@ def attention_small(q, k, v, out, B, heads, n_q, n_kv, d, ld_q, ld_k, ld_v, ld_o
     _count()
 
 
-# ---- dense prediction (the Depth Anything V2 DPT head) -------------------------------------------------------------
-def resize_bilinear(x, y, addend=None):
-    """F.interpolate(mode="bilinear", align_corners=True): x NHWC fp16 [N, H, W, C] -> y [N, Ho, Wo, C] (C % 8 == 0), with
-    ``addend`` (fp16, y's shape) added before the rounding; or fp32 single-channel maps x [N, H, W] -> y [N, Ho, Wo]."""
+# ---- dense prediction (the Depth Anything V2 DPT head, the UniFormer + UPerNet segmentor) ------------------------------
+def resize_bilinear(x, y, addend=None, align_corners=True):
+    """F.interpolate(mode="bilinear", align_corners=align_corners): x NHWC fp16 [N, H, W, C] -> y [N, Ho, Wo, C] (C % 8 == 0), with
+    ``addend`` (fp16, dense, y's shape; may be y) added before the rounding; y may be a channel slice of a wider NHWC buffer
+    (``cat[..., c0:c0 + C]``).  Or fp32 single-channel maps x [N, H, W] -> y [N, Ho, Wo] (align_corners=True only)."""
     _cuda(x, y, addend)
-    assert x.is_contiguous() and y.is_contiguous() and x.dtype == y.dtype
+    assert x.is_contiguous() and x.dtype == y.dtype
     if x.dtype == torch.float32:
+        assert align_corners and y.is_contiguous()
         assert x.dim() == 3 and y.dim() == 3 and addend is None and x.shape[0] == y.shape[0]
         N, H, W = x.shape
         _lib.check(_lib.load().anysd_resize_bilinear_ac_f32(_ptr(x), _ptr(y), N, H, W, y.shape[1], y.shape[2], _stream()),
                    "resize_bilinear")
     else:
         N, H, W, Cc = x.shape
-        assert x.dtype == torch.float16 and y.shape[0] == N and y.shape[3] == Cc
+        assert x.dtype == torch.float16 and y.dim() == 4 and y.shape[0] == N and y.shape[3] == Cc
+        ldy = y.stride(2)
+        assert y.stride(3) == 1 and y.stride(1) == y.shape[2] * ldy and y.stride(0) == y.shape[1] * y.stride(1), "y: NHWC rows ldy apart"
         if addend is not None:
             assert addend.shape == y.shape and addend.dtype == torch.float16 and addend.is_contiguous()
-        _lib.check(_lib.load().anysd_resize_bilinear_ac_f16(_ptr(x), _ptr(addend), _ptr(y), N, H, W, Cc, y.shape[1], y.shape[2],
-                                                            _stream()), "resize_bilinear")
+        _lib.check(_lib.load().anysd_resize_bilinear_f16(_ptr(x), _ptr(addend), _ptr(y), N, H, W, Cc, y.shape[1], y.shape[2], ldy,
+                                                         int(bool(align_corners)), _stream()), "resize_bilinear")
     _count()
 
 
@@ -483,6 +487,65 @@ def depth_to_space(g, out, r):
     assert g.is_contiguous() and out.is_contiguous() and g.dtype == out.dtype == torch.float16
     assert Ho % r == 0 and Wo % r == 0 and tuple(g.shape) == (B * (Ho // r) * (Wo // r), r * r * Cc)
     _lib.check(_lib.load().anysd_depth_to_space_f16(_ptr(g), _ptr(out), B, Ho // r, Wo // r, r, Cc, _stream()), "depth_to_space")
+    _count()
+
+
+def space_to_depth(x, g, r):
+    """x NHWC [B, H, W, C] (fp16 with C % 8 == 0, or a uint8 image) -> g fp16 [B*(H//r)*(W//r), r*r*C] with columns (ky, kx, c):
+    the rows of Conv2d(kernel = stride = r) as one contraction; the remainder rows / columns are cropped."""
+    _cuda(x, g)
+    B, H, W, Cc = x.shape
+    assert x.is_contiguous() and g.is_contiguous() and g.dtype == torch.float16 and x.dtype in (torch.float16, torch.uint8)
+    assert tuple(g.shape) == (B * (H // r) * (W // r), r * r * Cc)
+    fn = _lib.load().anysd_space_to_depth_f16 if x.dtype == torch.float16 else _lib.load().anysd_space_to_depth_u8
+    _lib.check(fn(_ptr(x), _ptr(g), B, H, W, Cc, r, _stream()), "space_to_depth")
+    _count()
+
+
+def dwconv(x, w, bias, y, residual=None):
+    """Depthwise Conv2d(C, C, k, padding=k // 2, groups=C) (+ residual): x, y, residual NHWC fp16 [N, H, W, C]; w fp32 [k*k, C]
+    (tap-major, see pack_dwconv), bias fp32 [C]."""
+    _cuda(x, w, bias, y, residual)
+    N, H, W, Cc = x.shape
+    k = int(round(w.shape[0] ** 0.5))
+    assert k * k == w.shape[0] and w.shape[1] == Cc and w.dtype == bias.dtype == torch.float32 and bias.numel() == Cc
+    assert x.dtype == y.dtype == torch.float16 and y.shape == x.shape and x.is_contiguous() and y.is_contiguous()
+    assert w.is_contiguous() and bias.is_contiguous()
+    if residual is not None:
+        assert residual.shape == x.shape and residual.dtype == torch.float16 and residual.is_contiguous()
+    _lib.check(_lib.load().anysd_dwconv_f16(_ptr(x), _ptr(w), _ptr(bias), _ptr(residual), _ptr(y), N, H, W, Cc, k, _stream()), "dwconv")
+    _count()
+
+
+def pack_dwconv(weight, dev):
+    """Depthwise Conv2d weight [C, 1, k, k] -> fp32 [k*k, C], the layout of ``dwconv``."""
+    C_, _, k, _ = weight.shape
+    return weight.detach().to(device=dev, dtype=torch.float32).reshape(C_, k * k).t().contiguous()
+
+
+def adaptive_avg_pool(x, y):
+    """nn.AdaptiveAvgPool2d(y's (Ho, Wo)) on NHWC fp16: x [N, H, W, C] -> y [N, Ho, Wo, C], C % 8 == 0."""
+    _cuda(x, y)
+    N, H, W, Cc = x.shape
+    assert x.dtype == y.dtype == torch.float16 and x.is_contiguous() and y.is_contiguous() and y.shape[0] == N and y.shape[3] == Cc
+    _lib.check(_lib.load().anysd_adaptive_avg_pool_f16(_ptr(x), _ptr(y), N, H, W, Cc, y.shape[1], y.shape[2], _stream()),
+               "adaptive_avg_pool")
+    _count()
+
+
+def seg_labels(logits, classes, mid_size, labels, palette=None, rgb=None):
+    """mmseg's labels: argmax over the first ``classes`` channels of resize(resize(logits, mid_size), labels' size), both resizes
+    half-pixel, per output pixel in fp32.  logits fp32 NHWC [N, h, w, ldl] (ldl % 4 == 0); labels int64 [N, Ho, Wo];
+    ``palette`` uint8 [classes, 3] with ``rgb`` uint8 [N, Ho, Wo, 3]: rgb = palette[label]."""
+    _cuda(logits, labels, palette, rgb)
+    N, h, w, ldl = logits.shape
+    assert logits.dtype == torch.float32 and logits.is_contiguous() and labels.dtype == torch.int64 and labels.is_contiguous()
+    assert labels.dim() == 3 and labels.shape[0] == N and 0 < classes <= ldl
+    if palette is not None or rgb is not None:
+        assert palette.dtype == rgb.dtype == torch.uint8 and palette.is_contiguous() and rgb.is_contiguous()
+        assert tuple(palette.shape) == (classes, 3) and tuple(rgb.shape) == (*labels.shape, 3)
+    _lib.check(_lib.load().anysd_seg_labels_f32(_ptr(logits), N, h, w, ldl, classes, int(mid_size[0]), int(mid_size[1]), labels.shape[1],
+                                                labels.shape[2], _ptr(labels), _ptr(palette), _ptr(rgb), _stream()), "seg_labels")
     _count()
 
 

@@ -256,12 +256,16 @@ int anysd_attention_small_f16(const void* q, const void* k, const void* v, void*
                               int ld_q, int ld_k, int ld_v, int ld_o, float scale, int causal, anysd_stream_t stream);
 
 /* ==== dense prediction: the Depth Anything V2 DPT head (AnyEdit_Collection/other_modules/depth_anything_v2/dpt.py,
- * util/blocks.py); its 1x1 / 3x3 convolutions and projections run on anysd_gemm_f16 ========================================
- * F.interpolate(x, (Ho, Wo), mode="bilinear", align_corners=True) on NHWC fp16 [N, H, W, C] -> y [N, Ho, Wo, C], any sizes,
- * C % 8 == 0; src = dst (in - 1) / (out - 1) in fp32 as ATen computes it.  addend (fp16 [N, Ho, Wo, C]) or NULL: added in fp32
- * before the one rounding (the FeatureFusionBlock sum `path + layer_rn`, blocks.py:132-134). */
-int anysd_resize_bilinear_ac_f16(const void* x, const void* addend, void* y, int N, int H, int W, int C, int Ho, int Wo,
-                                 anysd_stream_t stream);
+ * util/blocks.py) and the UniFormer + UPerNet segmentor (other_modules/uniformer/mmseg: backbones/uniformer.py,
+ * decode_heads/uper_head.py, psp_head.py); their 1x1 / 3x3 convolutions and projections run on anysd_gemm_f16 ===============
+ * F.interpolate(x, (Ho, Wo), mode="bilinear", align_corners) on NHWC fp16 [N, H, W, C] -> y [N, Ho, Wo, C], any sizes, C % 8 == 0,
+ * source coordinates in fp32 as ATen computes them: align_corners = 1: src = dst (in - 1) / (out - 1); 0 (half-pixel):
+ * src = max(in / out (dst + 0.5) - 0.5, 0); the upper neighbour is clamped to the edge.  y's pixels are ldy (>= C, % 8 == 0)
+ * elements apart, so y may be a channel slice of a concat buffer.  addend (dense fp16 [N, Ho, Wo, C], may be y itself when
+ * ldy == C) or NULL: added in fp32 before the one rounding (the FeatureFusionBlock sum `path + layer_rn`, blocks.py:132-134;
+ * UPerHead's top-down `laterals[i - 1] += resize(laterals[i])`). */
+int anysd_resize_bilinear_f16(const void* x, const void* addend, void* y, int N, int H, int W, int C, int Ho, int Wo, int ldy,
+                              int align_corners, anysd_stream_t stream);
 /* the same on fp32 single-channel maps [N, H, W] -> [N, Ho, Wo] (DepthAnythingV2.infer_image, dpt.py:192) */
 int anysd_resize_bilinear_ac_f32(const float* x, float* y, int N, int H, int W, int Ho, int Wo, anysd_stream_t stream);
 /* y = max(x, 0) into a separate buffer (ResidualConvUnit, blocks.py:70-71: x stays the residual); fp16, n % 8 == 0 */
@@ -270,6 +274,28 @@ int anysd_relu_f16(const void* x, void* y, long long n, anysd_stream_t stream);
  * [(ky, kx, co), ci] (bias repeated r^2 times) giving g [B gh gw, r r C], then this re-layout:
  * out[b, y r + ky, x r + kx, c] = g[(b gh + y) gw + x, (ky r + kx) C + c]; fp16, C % 8 == 0. */
 int anysd_depth_to_space_f16(const void* g, void* out, int B, int gh, int gw, int r, int C, anysd_stream_t stream);
+/* Conv2d(kernel = stride = r, padding 0) as one contraction (UniFormer PatchEmbed, uniformer.py:213-233): the inverse of
+ * depth_to_space with cropping, g[(b Ho + y) Wo + x, (ky r + kx) C + c] = in[b, y r + ky, x r + kx, c], Ho = H / r, Wo = W / r
+ * (rows / columns past the last whole patch are dropped, as the conv floors).  _f16: NHWC fp16, C % 8 == 0; _u8: a uint8 HWC
+ * image with any C, written as fp16 (exact). */
+int anysd_space_to_depth_f16(const void* in, void* g, int B, int H, int W, int C, int r, anysd_stream_t stream);
+int anysd_space_to_depth_u8(const void* in, void* g, int B, int H, int W, int C, int r, anysd_stream_t stream);
+/* Depthwise Conv2d(C, C, k, padding = k / 2, groups = C), k = 3 or 5 (UniFormer pos_embed and the CBlock's `attn`), NHWC fp16
+ * [N, H, W, C], C % 8 == 0: y = sum over taps (ky, kx) of w[ky k + kx, c] x + bias[c] (+ residual), fp32 accumulation, one
+ * rounding.  w fp32 [k k, C], bias fp32 [C]; residual fp16 like x or NULL (it may be x); y must not alias x. */
+int anysd_dwconv_f16(const void* x, const float* w, const float* bias, const void* residual, void* y, int N, int H, int W, int C,
+                     int k, anysd_stream_t stream);
+/* nn.AdaptiveAvgPool2d((Ho, Wo)) on NHWC fp16, C % 8 == 0 (the PPM of UPerHead, psp_head.py:36-55): output cell (i, j) averages
+ * rows [floor(i H / Ho), ceil((i + 1) H / Ho)) and likewise for columns, as ATen bins them (overlapping when Ho does not divide
+ * H, also when H < Ho); fp32 sum, one rounding. */
+int anysd_adaptive_avg_pool_f16(const void* x, void* y, int N, int H, int W, int C, int Ho, int Wo, anysd_stream_t stream);
+/* The labels of mmseg's whole-image test (encoder_decoder.py:84-94, 214-279): logits fp32 [N, h, w, ldl] (classes in the first
+ * `classes` columns, ldl % 4 == 0) resized half-pixel to the network input (Hm, Wm), that resized half-pixel to the original
+ * image (Ho, Wo), then argmax over the classes (the first maximum; softmax is monotonic) -> labels int64 [N, Ho, Wo].  Both
+ * resizes are evaluated per output pixel in fp32 in ATen's expression order; neither resized volume is stored.
+ * palette uint8 [classes, 3] and rgb uint8 [N, Ho, Wo, 3], both or neither: rgb = palette[label] (show_result at opacity 1). */
+int anysd_seg_labels_f32(const float* logits, int N, int h, int w, int ldl, int classes, int Hm, int Wm, int Ho, int Wo,
+                         long long* labels, const void* palette, void* rgb, anysd_stream_t stream);
 
 /* ==== training step (SURVEY.md a24; train.py:629-710) =====================================================
  * The reference back-propagates mse_loss(MoE(...), noise) through the frozen UNet with torch autograd
