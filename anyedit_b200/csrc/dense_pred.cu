@@ -13,6 +13,10 @@
 //   adaptive_avg_pool    nn.AdaptiveAvgPool2d with PyTorch's bins, NHWC fp16
 //   seg_labels           mmseg's two half-pixel resizes of the logits (to the network input, then to the original image) and
 //                        the argmax over classes, per original pixel, without the two fp32 logit volumes; optional palette
+//   hed_input            the HED edge network's (other_modules/HED/__init__.py) first 3x3 conv input as K = 32 im2col rows
+//   max_pool2            F.max_pool2d(2, 2) on NHWC fp16, bit-exact
+//   hed_edges            HEDdetector's post-processing: cv2's INTER_LINEAR resize of the five side maps, the mean, the fp64
+//                        sigmoid and the inversion to uint8, per output pixel
 #include "common.cuh"
 
 namespace anysd {
@@ -292,6 +296,127 @@ __global__ void seg_labels_kernel(const float* __restrict__ logits, int h, int w
     }
 }
 
+// HED's first conv as one K = 32 contraction: the im2col row of pixel (n, y, x) of a uint8 HWC image (3 channels in the image's
+// order), column (ky 3 + kx) 3 + c = fp16(s (img[n, y + ky - 1, x + kx - 1, c] - norm[c])) computed in fp32, zero outside the image
+// (the reference pads h = x - norm, after the subtraction) and in columns 27..31.  One pixel (four 16-byte vectors) per thread.
+__global__ void hed_input_kernel(const uint8_t* __restrict__ img, const float* __restrict__ norm, uint4* __restrict__ cols, int H, int W,
+                                 float s, long long total) {
+    const float m[3] = {norm[0], norm[1], norm[2]};
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+        const int x = (int)(i % W);
+        const long long r = i / W;
+        const int y = (int)(r % H);
+        const long long n = r / H;
+        __align__(16) __half v[32];
+#pragma unroll
+        for (int ky = 0; ky < 3; ++ky) {
+            const int iy = y + ky - 1;
+#pragma unroll
+            for (int kx = 0; kx < 3; ++kx) {
+                const int ix = x + kx - 1;
+                const bool in = iy >= 0 && iy < H && ix >= 0 && ix < W;
+                const uint8_t* p = img + ((n * H + iy) * W + ix) * 3;
+#pragma unroll
+                for (int c = 0; c < 3; ++c)
+                    v[(ky * 3 + kx) * 3 + c] = in ? __float2half_rn(((float)p[c] - m[c]) * s) : __float2half_rn(0.0f);
+            }
+        }
+#pragma unroll
+        for (int j = 27; j < 32; ++j) v[j] = __float2half_rn(0.0f);
+        const uint4* src = reinterpret_cast<const uint4*>(v);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) cols[i * 4 + j] = src[j];
+    }
+}
+
+// F.max_pool2d(kernel 2, stride 2) (floor: a last odd row / column is dropped) on NHWC fp16, 8 channels per thread.  The window is
+// scanned in ATen's order and a value replaces the running maximum when it is greater or NaN, so the result is one of the inputs,
+// bit for bit as ATen picks it.
+__device__ __forceinline__ uint32_t hmax2_first(uint32_t m, uint32_t v) {
+    const __half2 a = *reinterpret_cast<const __half2*>(&m), b = *reinterpret_cast<const __half2*>(&v);
+    const bool lo = __hgt(__low2half(b), __low2half(a)) || __hisnan(__low2half(b));
+    const bool hi = __hgt(__high2half(b), __high2half(a)) || __hisnan(__high2half(b));
+    return (lo ? (v & 0xFFFFu) : (m & 0xFFFFu)) | (hi ? (v & 0xFFFF0000u) : (m & 0xFFFF0000u));
+}
+__global__ void max_pool2_f16_kernel(const uint4* __restrict__ x, uint4* __restrict__ y, int H, int W, int Ho, int Wo, int CV,
+                                     long long total) {
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+        const int cv = (int)(i % CV);
+        long long r = i / CV;
+        const int ox = (int)(r % Wo);
+        r /= Wo;
+        const int oy = (int)(r % Ho);
+        const long long n = r / Ho;
+        const uint4* p = x + ((n * H + 2 * oy) * W + 2 * ox) * CV + cv;
+        const long long row = (long long)W * CV;
+        uint4 m = p[0];
+        const uint4 t[3] = {p[CV], p[row], p[row + CV]};
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+            m.x = hmax2_first(m.x, t[k].x);
+            m.y = hmax2_first(m.y, t[k].y);
+            m.z = hmax2_first(m.z, t[k].z);
+            m.w = hmax2_first(m.w, t[k].w);
+        }
+        y[i] = m;
+    }
+}
+
+// HED's post-processing (the reference's HEDdetector.__call__) per output pixel: each of the five fp32 side maps resized to (H, W) as
+// cv2.resize(INTER_LINEAR) does on float images (resize.cpp: scale = 1 / (out / in) and src = (dst + 0.5) scale - 0.5 in double,
+// rounded to float, floored, clamped to the edge; weights (1 - f, f); the horizontal pass, then the vertical one, each product and
+// sum rounded to fp32; a map of the output's size is copied), the mean in numpy's order (((((e0 + e1) + e2) + e3) + e4) / 5 in fp32,
+// then 1 / (1 + exp(-m)) in fp64, times 255, clipped, truncated to uint8 and inverted (cv2.bitwise_not).  Map k: pixel (n, y, x) at
+// p[k][((n h + y) w + x) ld].
+struct HedMaps {
+    const float* p[5];
+    int h[5], w[5];
+    double sh[5], sw[5];
+};
+struct CvTap {
+    int i0, i1;
+    float f;
+};
+__device__ __forceinline__ CvTap cv_tap(int d, double scale, int in) {
+    float f = (float)__dadd_rn(__dmul_rn((double)d + 0.5, scale), -0.5);
+    int s = (int)floorf(f);
+    f = __fsub_rn(f, (float)s);
+    if (s < 0) f = 0.0f, s = 0;
+    if (s >= in - 1) f = 0.0f, s = in - 1;
+    return CvTap{s, s + 1 < in ? s + 1 : s, f};
+}
+__global__ void hed_edges_kernel(HedMaps m, int ld, int H, int W, uint8_t* __restrict__ out, long long total) {
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+        const int x = (int)(i % W);
+        const long long r = i / W;
+        const int y = (int)(r % H);
+        const long long n = r / H;
+        float sum = 0.0f;
+#pragma unroll
+        for (int k = 0; k < 5; ++k) {
+            const int h = m.h[k], w = m.w[k];
+            const float* img = m.p[k] + n * h * w * (long long)ld;
+            float e;
+            if (h == H && w == W) {
+                e = img[((long long)y * w + x) * ld];
+            } else {
+                const CvTap ty = cv_tap(y, m.sh[k], h), tx = cv_tap(x, m.sw[k], w);
+                const float a0 = __fsub_rn(1.0f, tx.f), b0 = __fsub_rn(1.0f, ty.f);
+                const float* r0 = img + (long long)ty.i0 * w * ld;
+                const float* r1 = img + (long long)ty.i1 * w * ld;
+                const float h0 = __fadd_rn(__fmul_rn(r0[(long long)tx.i0 * ld], a0), __fmul_rn(r0[(long long)tx.i1 * ld], tx.f));
+                const float h1 = __fadd_rn(__fmul_rn(r1[(long long)tx.i0 * ld], a0), __fmul_rn(r1[(long long)tx.i1 * ld], tx.f));
+                e = __fadd_rn(__fmul_rn(h0, b0), __fmul_rn(h1, ty.f));
+            }
+            sum = k == 0 ? e : __fadd_rn(sum, e);
+        }
+        const float mean = __fdiv_rn(sum, 5.0f);
+        double v = __dmul_rn(__ddiv_rn(1.0, __dadd_rn(1.0, exp(-(double)mean))), 255.0);
+        v = v < 0.0 ? 0.0 : (v > 255.0 ? 255.0 : v);
+        out[i] = (uint8_t)(255 - (int)v);
+    }
+}
+
 static int dp_grid(long long n, int block = 256, int per_sm = 8) {
     long long g = (n + block - 1) / block;
     const long long cap = (long long)sm_count() * per_sm;
@@ -417,6 +542,46 @@ int anysd_seg_labels_f32(const float* logits, int N, int h, int w, int ldl, int 
         logits, h, w, ldl, classes, Hm, Wm, Ho, Wo, bl_scale(h, Hm, false), bl_scale(w, Wm, false), bl_scale(Hm, Ho, false),
         bl_scale(Wm, Wo, false), labels, (const uint8_t*)palette, (uint8_t*)rgb, total);
     return check_launch("seg_labels");
+}
+
+int anysd_hed_input_u8(const void* img, const float* norm, void* cols, int B, int H, int W, float scale, anysd_stream_t stream) {
+    ANYSD_REQUIRE(img && norm && cols, ANYSD_EINVAL, "hed_input: null pointer");
+    ANYSD_REQUIRE(B > 0 && H > 0 && W > 0, ANYSD_EINVAL, "hed_input: bad dims B=%d %dx%d", B, H, W);
+    ANYSD_REQUIRE((uintptr_t)cols % 16 == 0, ANYSD_EINVAL, "hed_input: cols must be 16-byte aligned");
+    const long long total = (long long)B * H * W;
+    hed_input_kernel<<<dp_grid(total), 256, 0, (cudaStream_t)stream>>>((const uint8_t*)img, norm, (uint4*)cols, H, W, scale, total);
+    return check_launch("hed_input");
+}
+
+int anysd_max_pool2_f16(const void* x, void* y, int N, int H, int W, int C, anysd_stream_t stream) {
+    ANYSD_REQUIRE(x && y, ANYSD_EINVAL, "max_pool2: null pointer");
+    ANYSD_REQUIRE(N > 0 && H >= 2 && W >= 2 && C > 0 && C % 8 == 0, ANYSD_EINVAL,
+                  "max_pool2: bad dims N=%d %dx%d C=%d (H, W >= 2; C must be a multiple of 8)", N, H, W, C);
+    ANYSD_REQUIRE((uintptr_t)x % 16 == 0 && (uintptr_t)y % 16 == 0, ANYSD_EINVAL, "max_pool2: pointers must be 16-byte aligned");
+    const int Ho = H / 2, Wo = W / 2;
+    const long long total = (long long)N * Ho * Wo * (C / 8);
+    max_pool2_f16_kernel<<<dp_grid(total), 256, 0, (cudaStream_t)stream>>>((const uint4*)x, (uint4*)y, H, W, Ho, Wo, C / 8, total);
+    return check_launch("max_pool2");
+}
+
+int anysd_hed_edges_u8(const float* const* maps, const int* sizes, int ld, int N, int H, int W, void* out, anysd_stream_t stream) {
+    ANYSD_REQUIRE(maps && sizes && out, ANYSD_EINVAL, "hed_edges: null pointer");
+    ANYSD_REQUIRE(N > 0 && H > 0 && W > 0 && ld > 0, ANYSD_EINVAL, "hed_edges: bad dims N=%d %dx%d ld=%d", N, H, W, ld);
+    HedMaps m;
+    for (int k = 0; k < 5; ++k) {
+        m.p[k] = maps[k];
+        m.h[k] = sizes[2 * k];
+        m.w[k] = sizes[2 * k + 1];
+        ANYSD_REQUIRE(m.p[k] && m.h[k] > 0 && m.w[k] > 0, ANYSD_EINVAL, "hed_edges: side map %d is null or empty (%dx%d)", k, m.h[k],
+                      m.w[k]);
+        ANYSD_REQUIRE((uintptr_t)m.p[k] % 4 == 0, ANYSD_EINVAL, "hed_edges: side map %d must be 4-byte aligned", k);
+        // cv2 resize.cpp: inv_scale = (double)dsize / ssize, scale = 1. / inv_scale
+        m.sh[k] = 1.0 / ((double)H / m.h[k]);
+        m.sw[k] = 1.0 / ((double)W / m.w[k]);
+    }
+    const long long total = (long long)N * H * W;
+    hed_edges_kernel<<<dp_grid(total), 256, 0, (cudaStream_t)stream>>>(m, ld, H, W, (uint8_t*)out, total);
+    return check_launch("hed_edges");
 }
 
 }  // extern "C"

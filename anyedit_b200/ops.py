@@ -549,6 +549,45 @@ def seg_labels(logits, classes, mid_size, labels, palette=None, rgb=None):
     _count()
 
 
+def hed_input(img, norm, cols, scale):
+    """HED's first conv input as K = 32 im2col rows: uint8 HWC img [B, H, W, 3], norm fp32 [3] -> cols fp16 [B*H*W, 32],
+    column (ky*3 + kx)*3 + c = fp16(scale * (img[.., y+ky-1, x+kx-1, c] - norm[c])), zero outside the image and in columns 27..31."""
+    _cuda(img, norm, cols)
+    B, H, W, Cc = img.shape
+    assert img.dtype == torch.uint8 and Cc == 3 and img.is_contiguous()
+    assert norm.dtype == torch.float32 and norm.numel() == 3 and norm.is_contiguous()
+    assert cols.dtype == torch.float16 and cols.is_contiguous() and tuple(cols.shape) == (B * H * W, 32)
+    _lib.check(_lib.load().anysd_hed_input_u8(_ptr(img), _ptr(norm), _ptr(cols), B, H, W, float(scale), _stream()), "hed_input")
+    _count()
+
+
+def max_pool2(x, y):
+    """F.max_pool2d(kernel_size=2, stride=2) on NHWC fp16: x [N, H, W, C] -> y [N, H // 2, W // 2, C], C % 8 == 0, bit-exact."""
+    _cuda(x, y)
+    N, H, W, Cc = x.shape
+    assert x.dtype == y.dtype == torch.float16 and x.is_contiguous() and y.is_contiguous()
+    assert tuple(y.shape) == (N, H // 2, W // 2, Cc)
+    _lib.check(_lib.load().anysd_max_pool2_f16(_ptr(x), _ptr(y), N, H, W, Cc, _stream()), "max_pool2")
+    _count()
+
+
+def hed_edges(maps, out):
+    """HEDdetector's post-processing: five fp32 side maps [N, h_k, w_k] (each may be a strided view of one column of an
+    [N, h_k, w_k, ld] buffer, the same ld for all) -> out uint8 [N, H, W] = 255 - uint8(255 sigmoid(mean of the cv2-resized maps))."""
+    _cuda(out, *maps)
+    assert len(maps) == 5 and out.dtype == torch.uint8 and out.is_contiguous() and out.dim() == 3
+    N, H, W = out.shape
+    ld = maps[0].stride(2)
+    for m in maps:
+        assert m.dtype == torch.float32 and m.dim() == 3 and m.shape[0] == N
+        assert m.stride(2) == ld and m.stride(1) == m.shape[2] * ld and m.stride(0) == m.shape[1] * m.stride(1), "maps: pixels ld apart"
+    ptrs = (C.c_void_p * 5)(*[m.data_ptr() for m in maps])
+    sizes = (C.c_int * 10)(*[d for m in maps for d in m.shape[1:]])
+    _lib.check(_lib.load().anysd_hed_edges_u8(C.cast(ptrs, C.c_void_p), C.cast(sizes, C.c_void_p), ld, N, H, W, _ptr(out), _stream()),
+               "hed_edges")
+    _count()
+
+
 # ---- training step (SURVEY.md a24): thin wrappers, same conventions as above -------------------------------------
 def q_sample(x0, noise, t, sqrt_acp, sqrt_1m_acp, out):
     _cuda(x0, noise, t, out)

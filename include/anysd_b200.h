@@ -296,6 +296,18 @@ int anysd_adaptive_avg_pool_f16(const void* x, void* y, int N, int H, int W, int
  * palette uint8 [classes, 3] and rgb uint8 [N, Ho, Wo, 3], both or neither: rgb = palette[label] (show_result at opacity 1). */
 int anysd_seg_labels_f32(const float* logits, int N, int h, int w, int ldl, int classes, int Hm, int Wm, int Ho, int Wo,
                          long long* labels, const void* palette, void* rgb, anysd_stream_t stream);
+/* The HED scribble annotator (other_modules/HED/__init__.py).  Its first 3x3 conv as one K = 32 contraction: from a uint8 HWC image
+ * [B, H, W, 3] (channels in the image's order), im2col rows cols fp16 [B H W, 32] with column (ky 3 + kx) 3 + c =
+ * fp16(scale (img[b, y + ky - 1, x + kx - 1, c] - norm[c])) computed in fp32, zero outside the image (padding after the
+ * subtraction, as the reference) and in columns 27..31.  norm: fp32 [3] on the device. */
+int anysd_hed_input_u8(const void* img, const float* norm, void* cols, int B, int H, int W, float scale, anysd_stream_t stream);
+/* F.max_pool2d(kernel 2, stride 2) on NHWC fp16 [N, H, W, C] -> [N, H / 2, W / 2, C] (floor), C % 8 == 0; the maximum is picked
+ * as ATen picks it (first greatest in window order, NaN wins), so the output is bit-exact. */
+int anysd_max_pool2_f16(const void* x, void* y, int N, int H, int W, int C, anysd_stream_t stream);
+/* HEDdetector's post-processing: maps[k] (k < 5; host array of device pointers) is an fp32 side map [N, sizes[2k], sizes[2k+1]] with
+ * pixels ld floats apart; each is resized to (H, W) as cv2.resize(INTER_LINEAR) does on float images, the five are averaged in
+ * numpy's order in fp32, and out uint8 [N, H, W] = 255 - uint8(clip(255 / (1 + exp(-mean)), 0, 255)) with the sigmoid in fp64. */
+int anysd_hed_edges_u8(const float* const* maps, const int* sizes, int ld, int N, int H, int W, void* out, anysd_stream_t stream);
 
 /* ==== training step (SURVEY.md a24; train.py:629-710) =====================================================
  * The reference back-propagates mse_loss(MoE(...), noise) through the frozen UNet with torch autograd
