@@ -35,6 +35,22 @@ __device__ __forceinline__ float act_f(float v, int act) {
     return act == 1 ? silu_f(v) : (act == 3 ? gelu_erf_f(v) : (act == 4 ? quick_gelu_f(v) : (act == 6 ? fmaxf(v, 0.0f) : v)));
 }
 
+// Exact (erf) GELU  x Phi(x)  in 11 instructions: Phi(x) = 1 / (1 + 2^(-x P(x^2))) with a cubic P fitted (minimax on the ABSOLUTE
+// error of x Phi(x), x^2 clamped at 36 -- beyond it the logistic is saturated either way) to |err| < 1.2e-5 for all x: 1/40 of the
+// fp16 spacing at unit magnitude, 1/7 of it at the minimum of GELU (-0.17).  Used by the fp16-output epilogues of gemm_wgmma.cu
+// (the GEGLU contractions are issue-bound there) and by the fused feed-forward (feedforward_wgmma.cu);
+// tests/test_gpu_ops.py::test_gelu_epilogue_accuracy pins the bound against torch's erf GELU.
+__device__ __forceinline__ float p_gelu(float v) {
+    const float t = fminf(v * v, 36.0f);
+    float q = fmaf(t, 2.483638929e-05f, 7.36060983e-04f);
+    q = fmaf(q, t, -0.10598272654f);
+    q = fmaf(q, t, -2.30164716054f);
+    float e, r;
+    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(v * q));          // 2^(-x P(x^2))
+    asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(1.0f + e));
+    return v * r;
+}
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

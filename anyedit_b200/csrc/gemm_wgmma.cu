@@ -106,21 +106,6 @@ __device__ __forceinline__ void g_wg_bar(int id) { asm volatile("bar.sync %0, 12
 __device__ __forceinline__ void g_turn_wait(int c) { asm volatile("bar.sync %0, 256;" ::"r"(7 + c) : "memory"); }
 __device__ __forceinline__ void g_turn_pass(int c) { asm volatile("bar.arrive %0, 256;" ::"r"(8 - c) : "memory"); }
 
-// Exact (erf) GELU  x Phi(x)  in 11 instructions: Phi(x) = 1 / (1 + 2^(-x P(x^2))) with a cubic P fitted (minimax on the ABSOLUTE
-// error of x Phi(x), x^2 clamped at 36 -- beyond it the logistic is saturated either way) to |err| < 1.2e-5 for all x: 1/40 of the
-// fp16 spacing at unit magnitude, 1/7 of it at the minimum of GELU (-0.17).  Used by the fp16-output epilogues (the GEGLU
-// contractions are issue-bound there); tests/test_gpu_ops.py::test_gelu_epilogue_accuracy pins the bound against torch's erf GELU.
-__device__ __forceinline__ float p_gelu(float v) {
-    const float t = fminf(v * v, 36.0f);
-    float q = fmaf(t, 2.483638929e-05f, 7.36060983e-04f);
-    q = fmaf(q, t, -0.10598272654f);
-    q = fmaf(q, t, -2.30164716054f);
-    float e, r;
-    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(v * q));          // 2^(-x P(x^2))
-    asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(1.0f + e));
-    return v * r;
-}
-
 struct TileCoord {
     int nt;              // column tile (first column nt * BN)
     int m0;              // dense: first row

@@ -292,6 +292,25 @@ def gemm(A, W, out, bias=None, rowadd=None, rows_per_batch=0, residual=None, act
     return st
 
 
+def geglu_ff(x, w1, b1, w2t, b2, residual, out):
+    """out = residual + W2 GEGLU(W1 x + b1) + b2 in one launch (anysd_geglu_ff_f16): x, residual, out fp16 [M, 320];
+    w1 / b1 the chunk-permuted ff1 pack (unet.ff1_chunk_order), w2t fp16 [1280, 320] = W2^T.  Traced as one contraction
+    with the FLOPs of both products."""
+    _cuda(x, w1, b1, w2t, b2, residual, out)
+    Cc = x.shape[-1]
+    M = x.numel() // Cc
+    hidden = w2t.shape[0]
+    assert w1.shape == (2 * hidden, Cc) and w2t.shape == (hidden, Cc) and b1.numel() == 2 * hidden
+    assert b1.dtype == torch.float32 and b2.dtype == torch.float32 and b1.is_contiguous() and b2.is_contiguous()
+    assert w1.is_contiguous() and w2t.is_contiguous()
+    fl = 2.0 * M * (2 * hidden) * Cc + 2.0 * M * Cc * hidden
+    with _Traced("gemm", fl, f"ff-geglu M={M} C={Cc} hidden={hidden}"):
+        _lib.check(_lib.load().anysd_geglu_ff_f16(_ptr(x), x.stride(-2), _ptr(w1), _ptr(b1), _ptr(w2t), _ptr(b2),
+                                                  _ptr(residual), residual.stride(-2), _ptr(out), out.stride(-2), M, Cc,
+                                                  hidden, _stream()), "geglu_ff")
+    _count()
+
+
 def conv3x3(x, W, out, bias=None, rowadd=None, residual=None, stride=1, upsample=0, ld_rowadd=None,
             logical_cin=None, logical_cout=None, act=0, pad_rb=False, stats=False):
     """x NHWC fp16 [N,H,W,Cin]; W fp16 [Cout, 9*Cin] ((ky,kx,ci) K order); out [N*Ho*Wo, Cout].

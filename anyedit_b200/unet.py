@@ -159,6 +159,23 @@ class _Embedding(nn.Module):
 _LN_FOLD = os.environ.get("ANYSD_LN_FOLD", "0")[:1] == "1"
 
 
+FF_FUSED_C = 320                # channel width of the transformer blocks whose feed-forward runs as one kernel (ops.geglu_ff)
+
+
+def ff1_chunk_order(hidden, chunk=32):
+    """Row order of the fused feed-forward's ff1 pack (feedforward_wgmma.cu), as indices into the interleaved (a_j, gate_j)
+    pack: within each chunk of ``chunk`` outputs, packed pair P (rows 2P, 2P + 1) holds hidden unit
+    16 (i // 4) + (2q, 2q + 1, 2q + 8, 2q + 9)[i % 4] with i = P // 4, q = P % 4 -- the unit whose GEGLU value the kernel
+    needs at that accumulator position as the register A operand of the second product.  Each (a, gate) pair stays together."""
+    idx = []
+    for c in range(hidden // chunk):
+        for P in range(chunk):
+            i, q = divmod(P, 4)
+            u = c * chunk + 16 * (i // 4) + (2 * q, 2 * q + 1, 2 * q + 8, 2 * q + 9)[i % 4]
+            idx += [2 * u, 2 * u + 1]
+    return torch.tensor(idx, dtype=torch.long)
+
+
 def _h(t, dev):
     return t.detach().to(device=dev, dtype=torch.float16).contiguous()
 
@@ -428,6 +445,11 @@ class UNetModel(nn.Module):
                 b["ff1_w"] = _h(torch.stack([gw[:inner], gw[inner:]], 1).reshape(2 * inner, -1), dev)
                 b["ff1_b"] = _f(torch.stack([gb[:inner], gb[inner:]], 1).reshape(-1), dev)
                 b["ff2_w"], b["ff2_b"] = _h(tb.ff.net[2].weight, dev), _f(tb.ff.net[2].bias, dev)
+                if st.inner == FF_FUSED_C and inner == 4 * FF_FUSED_C:
+                    # the fused feed-forward's packs: ff1 rows in the kernel's chunk order, W2 transposed (hidden-major)
+                    perm = ff1_chunk_order(inner).to(dev)
+                    b["ff1p_w"], b["ff1p_b"] = b["ff1_w"][perm].contiguous(), b["ff1_b"][perm].contiguous()
+                    b["ff2t_w"] = b["ff2_w"].t().contiguous()
                 d["blocks"].append(b)
             return d
 
@@ -793,6 +815,11 @@ class UNetModel(nn.Module):
                 self._attn(b["attn2"], ln2, ctx, N, n, st, False, t2, t3, expert=True, q_pre=q_pre)
                 ln3 = torch.empty_like(t3)
                 ops.layernorm(t3, b["ln3_w"], b["ln3_b"], ln3)
+                if "ff1p_w" in b:
+                    # 320 channels: both products and GEGLU in one launch, the hidden activations never written
+                    t = torch.empty_like(t3)
+                    ops.geglu_ff(ln3, b["ff1p_w"], b["ff1p_b"], b["ff2t_w"], b["ff2_b"], t3, t)
+                    continue
                 ffh = torch.empty(M, b["ff2_w"].shape[1], dtype=torch.float16, device=dev)
                 ops.gemm(ln3, b["ff1_w"], ffh, bias=b["ff1_b"], act=2)
             t4 = torch.empty_like(t3)

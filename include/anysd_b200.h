@@ -167,6 +167,15 @@ int anysd_gemm_stats_slabs(const anysd_gemm_params* p);
  * sums are added in split order by whichever unit finishes last.  The result therefore depends neither on the batch nor on the
  * arrival order -- but a caller that withholds the scratch gets the unsplit summation order (differs in fp32 rounding). */
 size_t anysd_gemm_splitk_workspace_bytes(const anysd_gemm_params* p);
+/* The GEGLU feed-forward of a 320-channel transformer block (attention.py FeedForward + the block's residual) as one kernel
+ * whose hidden activations stay on chip: out = residual + W2 GEGLU(W1 x + b1) + b2, everything fp16 [M, C] with row pitches
+ * ldx / ldr / ldo (multiples of 8), fp32 biases.  w1: fp16 [2 hidden, C], the ff1 rows interleaved (a_j, gate_j) as for
+ * anysd_gemm_f16 act = 2 and then permuted within each chunk of 32 outputs (anyedit_b200.unet.ff1_chunk_order), b1 [2 hidden]
+ * likewise; w2t: fp16 [hidden, C] = W2^T; b2 [C] (may be NULL).  Bit-identical to anysd_gemm_f16(x, ff1, act 2) followed by
+ * anysd_gemm_f16(hidden, W2, + b2, + residual).  Only C = 320, hidden = 4 C; pointers 16-byte aligned (EUNSUPPORTED /
+ * EINVAL otherwise). */
+int anysd_geglu_ff_f16(const void* x, int ldx, const void* w1, const float* b1, const void* w2t, const float* b2,
+                       const void* residual, int ldr, void* out, int ldo, int M, int C, int hidden, anysd_stream_t stream);
 
 /* ---- attention ---------------------------------------------------------------------------
  * CrossAttention.forward (attention.py:163-194) / xformers memory_efficient_attention (:233):
