@@ -83,6 +83,50 @@ __device__ __forceinline__ uint4 pack8(const float* f) {
     return u;
 }
 
+// One LayerNorm row held by LPR lanes, lane l holding the row's 8-element vectors l, l + LPR, .. (f[i] = vector
+// l + i LPR, valid while < CV; s its sum, added in order while loading): the xor-shuffle tree LPR / 2 .. 1, two-pass exact variance
+// (layernorm_row_stats), then f becomes the normalised output (layernorm_row_apply).  layernorm_kernel (norm.cu) and the
+// fused cross-attention block (xattn_block_wgmma.cu) both call these, so their LayerNorms are one expression.
+template <int LPR, int VPL>
+__device__ __forceinline__ void layernorm_row_stats(const float (&f)[VPL][8], float s, int l, int CV, float eps,
+                                                    float& mean, float& rstd) {
+#pragma unroll
+    for (int o = LPR / 2; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    const float inv_c = 1.0f / (float)(CV * 8);
+    // rounded on its own: with CV a compile-time constant the compiler would otherwise fuse s * inv_c into each f - mean
+    mean = __fmul_rn(s, inv_c);
+    float q = 0.f;
+#pragma unroll
+    for (int i = 0; i < VPL; ++i)
+        if (l + i * LPR < CV) {
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                float d = f[i][j] - mean;
+                q += d * d;
+            }
+        }
+#pragma unroll
+    for (int o = LPR / 2; o > 0; o >>= 1) q += __shfl_xor_sync(0xffffffffu, q, o);
+    rstd = rsqrtf(q * inv_c + eps);
+}
+template <int LPR, int VPL>
+__device__ __forceinline__ void layernorm_row_apply(float (&f)[VPL][8], int l, int CV, const float* __restrict__ gamma,
+                                                    const float* __restrict__ beta, float mean, float rstd) {
+#pragma unroll
+    for (int i = 0; i < VPL; ++i) {
+        const int v = l + i * LPR;
+        if (v < CV) {
+            const float4* g4 = reinterpret_cast<const float4*>(gamma + v * 8);
+            const float4* b4 = reinterpret_cast<const float4*>(beta + v * 8);
+            float4 g0 = __ldg(g4), g1 = __ldg(g4 + 1), b0 = __ldg(b4), b1 = __ldg(b4 + 1);
+            float gg[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w};
+            float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
+#pragma unroll
+            for (int j = 0; j < 8; ++j) f[i][j] = (f[i][j] - mean) * rstd * gg[j] + bb[j];
+        }
+    }
+}
+
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
     return (uint32_t)__cvta_generic_to_shared(p);
 }

@@ -562,47 +562,20 @@ __global__ void layernorm_kernel(const uint4* __restrict__ x, const float* __res
     for (int i = 0; i < VPL; ++i) {
         const int v = l + i * LPR;
         if (v < CV) {
-            uint4 u = __ldg(xr + v);
-            unpack8(u, f[i]);
+            unpack8(__ldg(xr + v), f[i]);
 #pragma unroll
             for (int j = 0; j < 8; ++j) s += f[i][j];
         }
     }
-#pragma unroll
-    for (int o = LPR / 2; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-    const float inv_c = 1.0f / (float)(CV * 8);
-    const float mean = s * inv_c;
-    float q = 0.f;
-#pragma unroll
-    for (int i = 0; i < VPL; ++i) {
-        const int v = l + i * LPR;
-        if (v < CV) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                float d = f[i][j] - mean;
-                q += d * d;
-            }
-        }
-    }
-#pragma unroll
-    for (int o = LPR / 2; o > 0; o >>= 1) q += __shfl_xor_sync(0xffffffffu, q, o);
-    const float rstd = rsqrtf(q * inv_c + eps);
+    float mean, rstd;
+    layernorm_row_stats<LPR, VPL>(f, s, l, CV, eps, mean, rstd);
     if (!row_ok) return;
+    layernorm_row_apply<LPR, VPL>(f, l, CV, gamma, beta, mean, rstd);
     uint4* yr = y + row * CV;
 #pragma unroll
     for (int i = 0; i < VPL; ++i) {
         const int v = l + i * LPR;
-        if (v < CV) {
-            const float4* g4 = reinterpret_cast<const float4*>(gamma + v * 8);
-            const float4* b4 = reinterpret_cast<const float4*>(beta + v * 8);
-            float4 g0 = __ldg(g4), g1 = __ldg(g4 + 1), b0 = __ldg(b4), b1 = __ldg(b4 + 1);
-            float gg[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w};
-            float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-            float o[8];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) o[j] = (f[i][j] - mean) * rstd * gg[j] + bb[j];
-            yr[v] = pack8(o);
-        }
+        if (v < CV) yr[v] = pack8(f[i]);
     }
 }
 

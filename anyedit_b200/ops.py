@@ -311,6 +311,27 @@ def geglu_ff(x, w1, b1, w2t, b2, residual, out):
     _count()
 
 
+def xattn_block(a1, t, wo1, bo1, ln2_w, ln2_b, wq, kv, L, wo2, bo2, ln3_w, ln3_b, t2, t3, l3, n, heads, d, hs,
+                aux_cols=True, eps=1e-5):
+    """A 320-channel transformer block from the self-attention's output projection to the feed-forward's LayerNorm in one
+    launch (anysd_xattn_block_f16): t2 = a1 Wo1^T + bo1 + t, t3 = attn(LN2(t2) Wq^T, K, V) Wo2^T + bo2 + t2, l3 = LN3(t3).
+    a1, t, t2, t3, l3 fp16 [M, C] contiguous with n rows per image; kv the kept context projection [images * L, ld]
+    (K then V).  Traced as one contraction with the FLOPs of its products."""
+    _cuda(a1, t, wo1, bo1, ln2_w, ln2_b, wq, kv, wo2, bo2, ln3_w, ln3_b, t2, t3, l3)
+    Cc = a1.shape[-1]
+    M = a1.numel() // Cc
+    for x in (a1, t, t2, t3, l3, wo1, wo2, wq, bo1, bo2, ln2_w, ln2_b, ln3_w, ln3_b):
+        assert x.is_contiguous()
+    assert kv.stride(-1) == 1
+    B = M // n
+    fl = 2.0 * M * Cc * Cc * 2 + 2.0 * M * heads * d * Cc + 4.0 * B * heads * n * L * d
+    with _Traced("gemm", fl, f"xattn-block M={M} C={Cc} L={L}"):
+        _lib.check(_lib.load().anysd_xattn_block_f16(
+            _ptr(a1), _ptr(t), _ptr(wo1), _ptr(bo1), _ptr(ln2_w), _ptr(ln2_b), _ptr(wq), _ptr(kv), kv.stride(-2), _ptr(wo2),
+            _ptr(bo2), _ptr(ln3_w), _ptr(ln3_b), _ptr(t2), _ptr(t3), _ptr(l3), M, n, L, Cc, heads, d, hs, int(aux_cols),
+            float(eps), _stream()), "xattn_block")
+    _count()
+
 def conv3x3(x, W, out, bias=None, rowadd=None, residual=None, stride=1, upsample=0, ld_rowadd=None,
             logical_cin=None, logical_cout=None, act=0, pad_rb=False, stats=False):
     """x NHWC fp16 [N,H,W,Cin]; W fp16 [Cout, 9*Cin] ((ky,kx,ci) K order); out [N*Ho*Wo, Cout].

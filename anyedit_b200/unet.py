@@ -160,6 +160,7 @@ _LN_FOLD = os.environ.get("ANYSD_LN_FOLD", "0")[:1] == "1"
 
 
 FF_FUSED_C = 320                # channel width of the transformer blocks whose feed-forward runs as one kernel (ops.geglu_ff)
+XATTN_MAX_CTX = 80              # longest context the fused cross-attention block (ops.xattn_block) keeps on chip
 
 
 def ff1_chunk_order(hidden, chunk=32):
@@ -693,27 +694,45 @@ class UNetModel(nn.Module):
                     ops.gemm(xq, ln[1]["w"], q, bias=ln[1]["b"], ln=(ln[0], ln[1]["cs"], 1e-5))
                 else:
                     ops.gemm(xq, ad["q_w"], q)
-            # context K/V: constant over the steps of one sampling run, so the DDIM stepper keeps them (st["kvc"]:
-            # mode "fill" computes into persistent buffers, mode "use" skips the projection)
-            kvc, xl = st.get("kvc"), st.get("xl", 0)
-            if kvc is not None and kvc["mode"] == "use":
-                kv = kvc["bufs"][xl]
-            else:
-                have = kvc is not None and len(kvc["bufs"]) > xl
-                kv = kvc["bufs"][xl] if have else torch.empty(N * L, 2 * Cp, dtype=torch.float16, device=dev)
-                ops.gemm(ctx.view(N * L, -1), ad["kv_w"], kv, bias=ad["kv_b"])
-                if kvc is not None and not have:
-                    kvc["bufs"].append(kv)
-            st["xl"] = xl + 1
+            kv = self._context_kv(ad, ctx, N, st)
             ops.attention(q, kv, kv[:, Cp:], a, N, ad["heads"], n_q, L, ad["d"], Cp, 2 * Cp, 2 * Cp, C, head_stride=hs,
                           aux_cols=ad["aux"])
             if expert and st["anysd"] is not None and st["anysd"].get("experts") is not None:
                 st["anysd"]["experts"](st["layer"], q, a, N, n_q, ad["heads"], ad["d"], hs, ad["aux"])
             if expert:
                 st["layer"] += 1
+        if out is None:
+            return a
         if out_stats:
             out._ln = ops.row_stats_buffer(N * n_q, C, dev)
         ops.gemm(a, ad["o_w"], out, bias=ad["o_b"], residual=residual, row_stats=out._ln if out_stats else None)
+
+    @staticmethod
+    def _context_kv(ad, ctx, N, st):
+        """The cross-attention's context K/V [N * L, 2 Cp]: constant over the steps of one sampling run, so the DDIM stepper
+        keeps them (st["kvc"]: mode "fill" computes into persistent buffers, mode "use" skips the projection)."""
+        L, Cp = ctx.shape[1], ad["heads"] * ad["hs"]
+        kvc, xl = st.get("kvc"), st.get("xl", 0)
+        if kvc is not None and kvc["mode"] == "use":
+            kv = kvc["bufs"][xl]
+        else:
+            have = kvc is not None and len(kvc["bufs"]) > xl
+            kv = kvc["bufs"][xl] if have else torch.empty(N * L, 2 * Cp, dtype=torch.float16, device=ctx.device)
+            ops.gemm(ctx.view(N * L, -1), ad["kv_w"], kv, bias=ad["kv_b"])
+            if kvc is not None and not have:
+                kvc["bufs"].append(kv)
+        st["xl"] = xl + 1
+        return kv
+
+    @staticmethod
+    def _xattn_fused(b, ctx, n, st):
+        """True when the span from attn1's output projection to norm3 runs as one kernel (ops.xattn_block): 320 channels as
+        8 aux_cols heads of 40, a self-attention attn1, whole 128-row tiles per image, a context of at most 80 tokens, and
+        no expert stream adding into the cross-attention output before its projection."""
+        a2 = b["attn2"]
+        experts = st["anysd"] is not None and st["anysd"].get("experts") is not None
+        return ("ff1p_w" in b and b["self"] and not experts and ctx is not None and ctx.shape[1] <= XATTN_MAX_CTX
+                and n % 128 == 0 and a2["aux"] and (a2["heads"], a2["d"], a2["hs"]) == (8, 40, 48))
 
     @staticmethod
     def _ln_folded(b):
@@ -776,6 +795,25 @@ class UNetModel(nn.Module):
                 t, h = self._dup_rows(t), self._dup_rows(h)
                 N, M, share = 2 * N, 2 * M, False
             fold = _LN_FOLD and inner % 64 == 0
+            if not fold and self._xattn_fused(b, ctx, n, st):
+                # 320 channels: attn1's output projection through norm3 in one launch, then the fused feed-forward
+                ln = torch.empty_like(t)
+                ops.layernorm(t, b["ln1_w"], b["ln1_b"], ln)
+                a1 = self._attn(b["attn1"], ln, None, N, n, st, True, t, None)
+                if share:
+                    # shared CFG halves: widen before attn1's output projection (identical halves, bit-identical result)
+                    a1, t, h = self._dup_rows(a1), self._dup_rows(t), self._dup_rows(h)
+                    N, M, share = 2 * N, 2 * M, False
+                a1d, ad = b["attn1"], b["attn2"]
+                kv = self._context_kv(ad, ctx, N, st)
+                st["layer"] += 1
+                t2, t3, ln3 = (torch.empty_like(t) for _ in range(3))
+                ops.xattn_block(a1, t, a1d["o_w"], a1d["o_b"], b["ln2_w"], b["ln2_b"], ad["q_w"], kv, ctx.shape[1],
+                                ad["o_w"], ad["o_b"], b["ln3_w"], b["ln3_b"], t2, t3, ln3, n, ad["heads"], ad["d"], ad["hs"],
+                                aux_cols=ad["aux"])
+                t = torch.empty_like(t3)
+                ops.geglu_ff(ln3, b["ff1p_w"], b["ff1p_b"], b["ff2t_w"], b["ff2_b"], t3, t)
+                continue
             if fold:
                 # LayerNorm folded into the contractions either side of it (anysd_gemm_params::row_stats / ln_stats): the
                 # producer of t / t2 / t3 has left per-row moments, the consumer takes the un-normalised rows

@@ -176,6 +176,20 @@ size_t anysd_gemm_splitk_workspace_bytes(const anysd_gemm_params* p);
  * EINVAL otherwise). */
 int anysd_geglu_ff_f16(const void* x, int ldx, const void* w1, const float* b1, const void* w2t, const float* b2,
                        const void* residual, int ldr, void* out, int ldo, int M, int C, int hidden, anysd_stream_t stream);
+/* The span of a 320-channel transformer block from the self-attention's output projection to the feed-forward's
+ * LayerNorm as one kernel (attention.py BasicTransformerBlock :262-264 with CrossAttention :163-194 as attn2):
+ *   t2 = a1 Wo1^T + bo1 + t;  t3 = attn(LN2(t2) Wq^T, K, V) Wo2^T + bo2 + t2;  l3 = LN3(t3).
+ * a1, t, t2, t3, l3: fp16 [M, C] contiguous, M = images * n rows; wo1, wo2: fp16 [C, C]; wq: fp16 [heads * hs, C] with
+ * the aux_cols packing (heads padded to hs, scale * log2(e) folded in, no bias); kv: fp16 [images * L, ld_kv], K at
+ * columns [0, heads * hs), V after it, as anysd_gemm_f16 leaves the context projection with its aux_cols bias; biases
+ * and LayerNorm weights fp32 [C].  Bit-identical to anysd_gemm_f16 (+ bias + residual), anysd_layernorm_f16,
+ * anysd_gemm_f16, anysd_attention_f16 (aux_cols), anysd_gemm_f16 (+ bias + residual), anysd_layernorm_f16.
+ * Only C = 320 as 8 heads of d = 40 at stride 48 with aux_cols, n a multiple of 128, L <= 80 (EUNSUPPORTED otherwise);
+ * pointers 16-byte aligned (EINVAL). */
+int anysd_xattn_block_f16(const void* a1, const void* t, const void* wo1, const float* bo1, const float* ln2_w,
+                          const float* ln2_b, const void* wq, const void* kv, int ld_kv, const void* wo2, const float* bo2,
+                          const float* ln3_w, const float* ln3_b, void* t2, void* t3, void* l3, int M, int n, int L, int C,
+                          int heads, int d, int hs, int aux_cols, float eps, anysd_stream_t stream);
 
 /* ---- attention ---------------------------------------------------------------------------
  * CrossAttention.forward (attention.py:163-194) / xformers memory_efficient_attention (:233):
