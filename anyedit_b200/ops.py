@@ -628,6 +628,19 @@ def hed_edges(maps, out):
     _count()
 
 
+def sketch(images, out, low=50, high=150):
+    """img2sketch's Canny chain, equal to OpenCV on every pixel: uint8 BGR images [B, H, W, 3] -> out uint8 [B, H, W] =
+    255 - Canny(GaussianBlur(grey, (3, 3), 0), low, high).  Four launches; the label and flag scratch is allocated here."""
+    _cuda(images, out)
+    B, H, W, Cc = images.shape
+    assert images.dtype == torch.uint8 and Cc == 3 and images.is_contiguous()
+    assert out.dtype == torch.uint8 and out.is_contiguous() and tuple(out.shape) == (B, H, W)
+    lib = _lib.load()
+    ws = torch.empty((lib.anysd_sketch_workspace_bytes(B, H, W) + 3) // 4, dtype=torch.int32, device=images.device)
+    _lib.check(lib.anysd_sketch_u8(_ptr(images), B, H, W, int(low), int(high), _ptr(ws), _ptr(out), _stream()), "sketch")
+    _count(4)
+
+
 # ---- training step (SURVEY.md a24): thin wrappers, same conventions as above -------------------------------------
 def q_sample(x0, noise, t, sqrt_acp, sqrt_1m_acp, out):
     _cuda(x0, noise, t, out)

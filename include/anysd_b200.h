@@ -331,6 +331,13 @@ int anysd_max_pool2_f16(const void* x, void* y, int N, int H, int W, int C, anys
  * pixels ld floats apart; each is resized to (H, W) as cv2.resize(INTER_LINEAR) does on float images, the five are averaged in
  * numpy's order in fp32, and out uint8 [N, H, W] = 255 - uint8(clip(255 / (1 + exp(-mean)), 0, 255)) with the sigmoid in fp64. */
 int anysd_hed_edges_u8(const float* const* maps, const int* sizes, int ld, int N, int H, int W, void* out, anysd_stream_t stream);
+/* AnyEdit's Canny sketch annotator (visual_condition_tool.py img2sketch), equal to OpenCV on every pixel: img uint8 [B, H, W, 3] BGR
+ * -> out uint8 [B, H, W] = 255 - Canny(GaussianBlur(cvtColor(img, BGR2GRAY), (3, 3), 0), low, high) with the 3x3 aperture and the
+ * L1 gradient.  Hysteresis is union-find connected-component labelling in four launches whatever the image holds; workspace
+ * (anysd_sketch_workspace_bytes, 4-byte aligned) holds the int32 labels and the root flags, and needs no clearing.  Refuses
+ * low < 0, low > high and B H W > 2^31 - 1 (a label is a pixel index). */
+size_t anysd_sketch_workspace_bytes(int B, int H, int W);
+int anysd_sketch_u8(const void* img, int B, int H, int W, int low, int high, void* workspace, void* out, anysd_stream_t stream);
 
 /* ==== training step (SURVEY.md a24; train.py:629-710) =====================================================
  * The reference back-propagates mse_loss(MoE(...), noise) through the frozen UNet with torch autograd
