@@ -61,8 +61,8 @@ __global__ void silu_bwd_f32_kernel(const float* __restrict__ x, const float* __
 // y = [silu](z), z = xhat * gamma + beta, xhat = (x - mean) * rstd over the group's HW x cpg elements:
 //   dz = dy * silu'(z);  w = dz * gamma;  dx = rstd * (w - mean(w) - xhat * mean(w * xhat))
 // One thread-block CLUSTER per (image, span of `gpc` whole groups that is also a whole number of 16-byte channel vectors); the
-// cluster's CS CTAs split the HW rows, each with VC = gpc*cpg/8 vector columns x RL row lanes.  Three passes over the slab
-// (statistics; the two sums; dx), the slab stays in L2.  Per-channel partials are folded over the row lanes in smem, then per
+// cluster's CS CTAs split the HW rows, each with VC = gpc*cpg/8 vector columns x RL row lanes.  Four passes over the slab
+// (mean; centred squares; the two sums; dx), the slab stays in L2.  Per-channel partials are folded over the row lanes in smem, then per
 // group, then over the cluster through distributed shared memory in rank order (deterministic).  One CTA per slab would leave
 // the 64x64 level at 128 CTAs with one 16-byte load in flight per thread.
 constexpr int GNB_THREADS = 256;
@@ -153,25 +153,36 @@ __global__ void __launch_bounds__(GNB_THREADS) gn_bwd_kernel(const __half* __res
             float f[8];
             unpack8(__ldg(reinterpret_cast<const uint4*>(xb + (size_t)r * xs)), f);
 #pragma unroll
+            for (int j = 0; j < 8; ++j) a8[j] += f[j];
+        }
+    fold(a8, b8, 0, 1);                            // slot 0: mean (b8 is zero; slot 1 is rewritten below)
+    float mean8[8], rstd8[8], g8[8], be8[8];
+    if (active) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) mean8[j] = grp[((vl * 8 + j) / cpg) * 4];
+    }
+    // Two-pass variance from centred squares: E[x^2] - mean^2 in fp32 loses about kappa = E[x^2] / var ulps, which a group with
+    // a DC offset of 64 sigma (kappa = 4096) turns into a visible error in rstd and hence in dx.
+#pragma unroll
+    for (int j = 0; j < 8; ++j) a8[j] = 0.f;
+    if (active)
+#pragma unroll 4
+        for (int r = row_lo + rl; r < row_hi; r += RL) {
+            float f[8];
+            unpack8(__ldg(reinterpret_cast<const uint4*>(xb + (size_t)r * xs)), f);
+#pragma unroll
             for (int j = 0; j < 8; ++j) {
-                a8[j] += f[j];
-                b8[j] += f[j] * f[j];
+                const float d = f[j] - mean8[j];
+                a8[j] = fmaf(d, d, a8[j]);
             }
         }
-    fold(a8, b8, 0, 1);
-    if (threadIdx.x < gpc) {                       // slot 1 holds E[x^2] -> rstd
-        const float mean = grp[threadIdx.x * 4], ex2 = grp[threadIdx.x * 4 + 1];
-        float var = ex2 - mean * mean;
-        var = var < 0.f ? 0.f : var;
-        grp[threadIdx.x * 4 + 1] = rsqrtf(var + eps);
-    }
+    fold(a8, b8, 1, 2);                            // slot 1: variance (slot 2 is rewritten by the next fold)
+    if (threadIdx.x < gpc) grp[threadIdx.x * 4 + 1] = rsqrtf(grp[threadIdx.x * 4 + 1] + eps);
     __syncthreads();
-    float mean8[8], rstd8[8], g8[8], be8[8];
     if (active) {
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
             const int gl = (vl * 8 + j) / cpg;
-            mean8[j] = grp[gl * 4];
             rstd8[j] = grp[gl * 4 + 1];
             g8[j] = gamma[c0 + j];
             be8[j] = beta[c0 + j];

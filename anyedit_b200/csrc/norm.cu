@@ -583,6 +583,28 @@ __global__ void layernorm_kernel(const uint4* __restrict__ x, const float* __res
 
 using namespace anysd;
 
+// Workspace of W 4-byte words.  The persistent words sit at the FRONT, at offsets no call's shape moves: the one-launch path's
+// grid barrier {arrivals, generation} at words 0, 1 and image n's completion counter at word 2 + n (both must be zero on first
+// use; every launch re-arms them).  The scratch of a call -- partials [N, 64, G, 2] | mean/rstd [N, G, 2], 130 N G words --
+// sits at the END.  The size check asks for 131 N G + 2 <= W, so for any two accepted calls A and B
+//   130 N_A G_A <= 130 (W - 2) / 131   and   N_B + 2 <= (W - 2) / 131 + 2:
+// A's scratch never covers B's persistent words, and one workspace serves calls of any batch size and group count in any order.
+struct GnWorkspace {
+    unsigned int* bar;
+    unsigned int* counters;
+    float* partials;
+    float* meanrstd;
+};
+static GnWorkspace gn_workspace(void* ws, size_t bytes, int N, int G) {
+    GnWorkspace w;
+    const size_t words = bytes / sizeof(float);
+    w.bar = (unsigned int*)ws;
+    w.counters = w.bar + 2;
+    w.partials = (float*)ws + (words - (size_t)N * G * (GN_MAX_SPLITS * 2 + 2));
+    w.meanrstd = w.partials + (size_t)N * GN_MAX_SPLITS * G * 2;
+    return w;
+}
+
 extern "C" {
 
 int anysd_groupnorm_resident(int C1, int C2, int HW, int G) {
@@ -593,11 +615,9 @@ int anysd_groupnorm_resident(int C1, int C2, int HW, int G) {
 size_t anysd_groupnorm_workspace_bytes(int N, int G, int C) {
     (void)C;
     if (N <= 0 || G <= 0) return 0;
-    // partials [N, 64, G, 2] | mean/rstd [N, G, 2] | per-image completion counters [N] (must be zero on first use:
-    // the caller zero-fills the workspace once; every launch re-arms them)
-    // | grid barrier of the one-launch path {arrivals, generation}
-    return (size_t)N * GN_MAX_SPLITS * G * 2 * sizeof(float) + (size_t)N * G * 2 * sizeof(float) + (size_t)N * sizeof(unsigned int) +
-           2 * sizeof(unsigned int);
+    // scratch: partials [N, 64, G, 2] | mean/rstd [N, G, 2]; plus N * G + 2 words for the persistent words, of which N + 2 are
+    // used: the slack keeps every accepted call's scratch off every other call's persistent words (see gn_workspace)
+    return ((size_t)N * GN_MAX_SPLITS * G * 2 + (size_t)N * G * 2 + (size_t)N * G + 2) * sizeof(float);
 }
 
 int anysd_groupnorm_nhwc_f16(const void* x1, int C1, const void* x2, int C2, const float* gamma, const float* beta,
@@ -609,7 +629,8 @@ int anysd_groupnorm_nhwc_f16(const void* x1, int C1, const void* x2, int C2, con
     ANYSD_REQUIRE(N > 0 && HW > 0 && G > 0 && G <= 64 && C1 > 0 && C2 >= 0, ANYSD_EINVAL, "groupnorm: bad shape");
     ANYSD_REQUIRE(C % G == 0 && C1 % 8 == 0 && C2 % 8 == 0, ANYSD_EINVAL,
                   "groupnorm: C=%d must divide into G=%d groups and both sources must be multiples of 8 channels", C, G);
-    ANYSD_REQUIRE(C / 8 <= 1024, ANYSD_EINVAL, "groupnorm: C=%d too large", C);
+    // the statistics + apply kernels give one thread to each 16-byte channel vector of a row: C / 8 <= 512 threads
+    ANYSD_REQUIRE(C <= 4096, ANYSD_EUNSUPPORTED, "groupnorm: C=%d channels, at most 4096 are supported", C);
     ANYSD_REQUIRE(workspace_bytes >= anysd_groupnorm_workspace_bytes(N, G, C), ANYSD_EINVAL,
                   "groupnorm: workspace too small (%zu bytes)", workspace_bytes);
     const int cpg = C / G;
@@ -632,9 +653,7 @@ int anysd_groupnorm_nhwc_f16(const void* x1, int C1, const void* x2, int C2, con
         cudaError_t e = cudaFuncSetAttribute(gn_stats_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         ANYSD_REQUIRE(e == cudaSuccess, ANYSD_ECUDA, "groupnorm: smem opt-in failed: %s", cudaGetErrorString(e));
     }
-    float* partials = (float*)workspace;
-    float* meanrstd = partials + (size_t)N * GN_MAX_SPLITS * G * 2;
-    unsigned int* counters = (unsigned int*)(meanrstd + (size_t)N * G * 2);
+    const GnWorkspace w = gn_workspace(workspace, workspace_bytes, N, G);
     // One cooperative launch when the device can hold a useful grid (ANYSD_GN_FUSED=0 forces the two-kernel path,
     // which produces the same bits).
     static const char* fused_env = getenv("ANYSD_GN_FUSED");
@@ -654,8 +673,8 @@ int anysd_groupnorm_nhwc_f16(const void* x1, int C1, const void* x2, int C2, con
             GnFusedArgs fa;
             fa.x1 = (const uint4*)x1; fa.x2 = (const uint4*)x2;
             fa.CV = g.CV; fa.CV1 = g.CV1; fa.R = g.R; fa.HW = HW; fa.rows_per_block = rpb; fa.S = S; fa.N = N; fa.G = G; fa.cpg = cpg;
-            fa.eps = eps; fa.partials = partials; fa.gamma = gamma; fa.beta = beta; fa.fuse_silu = fuse_silu; fa.y = (uint4*)y;
-            fa.bar = counters + N;
+            fa.eps = eps; fa.partials = w.partials; fa.gamma = gamma; fa.beta = beta; fa.fuse_silu = fuse_silu; fa.y = (uint4*)y;
+            fa.bar = w.bar;
             void* kargs[] = {(void*)&fa};
             cudaError_t e = cudaLaunchCooperativeKernel((const void*)gn_fused_kernel, dim3((unsigned)P), dim3(g.T), kargs, smem, st);
             ANYSD_REQUIRE(e == cudaSuccess, ANYSD_ECUDA, "groupnorm (fused): launch failed: %s", cudaGetErrorString(e));
@@ -663,11 +682,11 @@ int anysd_groupnorm_nhwc_f16(const void* x1, int C1, const void* x2, int C2, con
         }
     }
     gn_stats_kernel<<<dim3(S, N), g.T, smem, st>>>((const uint4*)x1, (const uint4*)x2, g.CV, g.CV1, g.R, HW, rpb, G, cpg, eps,
-                                                   partials, meanrstd, counters);
+                                                   w.partials, w.meanrstd, w.counters);
     int rc = check_launch("groupnorm stats");
     if (rc) return rc;
     gn_apply_kernel<<<dim3(S, N), g.T, 0, st>>>((const uint4*)x1, (const uint4*)x2, g.CV, g.CV1, g.R, HW, rpb, G, cpg,
-                                                meanrstd, gamma, beta, fuse_silu, (uint4*)y);
+                                                w.meanrstd, gamma, beta, fuse_silu, (uint4*)y);
     return check_launch("groupnorm apply");
 }
 
@@ -675,8 +694,9 @@ int anysd_groupnorm_apply_nhwc_f16(const void* x, int C, const float* stats1, in
                                    const float* beta, void* y, int N, int HW, int G, float eps, int fuse_silu, void* workspace,
                                    size_t workspace_bytes, anysd_stream_t stream) {
     ANYSD_REQUIRE(x && stats1 && gamma && beta && y && workspace, ANYSD_EINVAL, "groupnorm_apply: null pointer");
-    ANYSD_REQUIRE(N > 0 && HW > 0 && G > 0 && G <= 64 && C > 0 && C % G == 0 && C % 8 == 0 && C / 8 <= 1024, ANYSD_EINVAL,
+    ANYSD_REQUIRE(N > 0 && HW > 0 && G > 0 && G <= 64 && C > 0 && C % G == 0 && C % 8 == 0, ANYSD_EINVAL,
                   "groupnorm_apply: bad shape N=%d HW=%d C=%d G=%d", N, HW, C, G);
+    ANYSD_REQUIRE(C <= 4096, ANYSD_EUNSUPPORTED, "groupnorm_apply: C=%d channels, at most 4096 are supported", C);
     ANYSD_REQUIRE(C1 > 0 && C1 <= C && (C1 == C) == (stats2 == nullptr), ANYSD_EINVAL,
                   "groupnorm_apply: stats2 must be given exactly when the first source covers fewer than C channels");
     ANYSD_REQUIRE(S > 0 && S * 32 == HW, ANYSD_EINVAL, "groupnorm_apply: S=%d slabs of 32 rows must cover HW=%d", S, HW);
@@ -690,7 +710,7 @@ int anysd_groupnorm_apply_nhwc_f16(const void* x, int C, const float* stats1, in
     const int rpb = batch * nb;
     const int Sx = cdiv(HW, rpb);
     cudaStream_t st = (cudaStream_t)stream;
-    float* meanrstd = (float*)workspace + (size_t)N * GN_MAX_SPLITS * G * 2;
+    float* meanrstd = gn_workspace(workspace, workspace_bytes, N, G).meanrstd;
     gn_finalize_kernel<<<dim3(G, N), 128, 0, st>>>((const float2*)stats1, C1, (const float2*)stats2, C - C1, S, HW, cpg, eps, meanrstd);
     int rc = check_launch("groupnorm finalize");
     if (rc) return rc;

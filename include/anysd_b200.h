@@ -79,8 +79,10 @@ int anysd_router_gate_f32(const float* table, const long long* idx, int table_ro
  * SpatialTransformer GroupNorm (attention.py:88-89, 326; eps 1e-6, no SiLU).  Statistics in fp32.
  * The input may be the channel concat of two NHWC tensors (x2 != NULL): the skip concat
  * (openaimodel.py:780) is then never materialised for the norm. y: NHWC fp16 [N, HW, C1+C2]. */
-/* The workspace must be zero-filled once before its first use (it holds per-image completion counters that every
- * launch re-arms); it may then be reused by any number of stream-ordered calls. */
+/* The workspace must be zero-filled once before its first use (it holds per-image completion counters and a grid barrier
+ * that every launch re-arms, at offsets that do not depend on the call's shape); it may then be reused by any number of
+ * stream-ordered calls whose anysd_groupnorm_workspace_bytes(N, G, C) it covers, in any order of N and G.
+ * C1 + C2 <= 4096 (ANYSD_EUNSUPPORTED otherwise), G <= 64. */
 size_t anysd_groupnorm_workspace_bytes(int N, int G, int C);
 int anysd_groupnorm_nhwc_f16(const void* x1, int C1, const void* x2, int C2, const float* gamma,
                              const float* beta, void* y, int N, int HW, int G, float eps, int fuse_silu,
