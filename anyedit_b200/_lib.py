@@ -103,7 +103,7 @@ SIGNATURES = {
     "anysd_gaussian_posterior_f32": (_I, [_VP, _VP, _VP, _VP, _F, _I, _LL, _VP]),
     "anysd_embed_tokens_f16": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, _I, _VP]),
     "anysd_attention_small_f16": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _I, _I, _I, _I, _F, _I, _VP]),
-    # ---- dense prediction (Depth Anything V2 head, UniFormer + UPerNet segmentor, HED, Canny sketch) ----
+    # ---- dense prediction (Depth Anything V2 head, UniFormer + UPerNet segmentor, HED, Canny sketch, AnyDoor) ----
     "anysd_resize_bilinear_f16": (_I, [_VP, _VP, _VP, _I, _I, _I, _I, _I, _I, _I, _I, _VP]),
     "anysd_resize_bilinear_ac_f32": (_I, [_VP, _VP, _I, _I, _I, _I, _I, _VP]),
     "anysd_relu_f16": (_I, [_VP, _VP, _LL, _VP]),
@@ -118,6 +118,11 @@ SIGNATURES = {
     "anysd_hed_edges_u8": (_I, [_VP, _VP, _I, _I, _I, _I, _VP, _VP]),
     "anysd_sketch_workspace_bytes": (_SZ, [_I, _I, _I]),
     "anysd_sketch_u8": (_I, [_VP, _I, _I, _I, _I, _I, _VP, _VP, _VP]),
+    "anysd_resize_linear_u8": (_I, [_VP, _I, _I, _I, _I, _VP, _I, _I, _VP]),
+    "anysd_anydoor_bbox_u8": (_I, [_VP, _I, _I, _I, _VP, _VP]),
+    "anysd_anydoor_prepare": (_I, [_VP, _VP, _I, _I, _VP, _I, _I, _I, _VP] + [_VP] * 9 + [_VP]),
+    "anysd_anydoor_sobel": (_I, [_VP, _VP, _I, _VP, _VP, _VP, _VP, _VP]),
+    "anysd_anydoor_crop_back": (_I, [_VP, _I, _VP, _I, _I, _I, _VP, _VP, _VP]),
     # ---- training step ----
     "anysd_q_sample_f32": (_I, [_VP, _VP, _VP, _VP, _VP, _VP, _I, _LL, _VP]),
     "anysd_mse_workspace_bytes": (_SZ, []),

@@ -641,6 +641,69 @@ def sketch(images, out, low=50, high=150):
     _count(4)
 
 
+
+def resize_linear_u8(src, dst):
+    """cv2.resize(INTER_LINEAR) of uint8 images, equal to OpenCV on every byte: src [B, H, W, C] -> dst [B, OH, OW, C]."""
+    _cuda(src, dst)
+    B, H, W, Cc = src.shape
+    assert src.dtype == dst.dtype == torch.uint8 and src.is_contiguous() and dst.is_contiguous()
+    assert dst.dim() == 4 and dst.shape[0] == B and dst.shape[3] == Cc
+    _lib.check(_lib.load().anysd_resize_linear_u8(_ptr(src), B, H, W, Cc, _ptr(dst), dst.shape[1], dst.shape[2], _stream()),
+               "resize_linear_u8")
+    _count()
+
+
+def anydoor_bbox(masks, out):
+    """uint8 masks [B, H, W] -> out int32 [B, 6] = (sum, first row, last row, first column, last column, largest value)."""
+    _cuda(masks, out)
+    B, H, W = masks.shape
+    assert masks.dtype == torch.uint8 and masks.is_contiguous() and out.dtype == torch.int32 and tuple(out.shape) == (B, 6)
+    _lib.check(_lib.load().anysd_anydoor_bbox_u8(_ptr(masks), B, H, W, _ptr(out), _stream()), "anydoor_bbox")
+    _count()
+
+
+def anydoor_prepare(ref_images, ref_masks, tar_images, geom, st):
+    """AnyDoor's process_pairs pixel work (five launches): uint8 [B, RH, RW, 3] reference images and their 0/1 masks
+    [B, RH, RW], uint8 [B, TH, TW, 3] target images, the
+    int32 [B, ANYDOOR_P] geometry -> the stage tensors of ``st`` (keys ref_u8, mask_u8, img256, m256, hf256, hf224, ref, jpg,
+    hint; shapes in include/anysd_b200.h)."""
+    keys = ("ref_u8", "mask_u8", "img256", "m256", "hf256", "hf224", "ref", "jpg", "hint")
+    _cuda(ref_images, ref_masks, tar_images, geom, *(st[k] for k in keys))
+    B, RH, RW, _ = ref_images.shape
+    TH, TW = tar_images.shape[1:3]
+    for t in (ref_images, ref_masks, tar_images, geom, *(st[k] for k in keys)):
+        assert t.is_contiguous() and t.shape[0] == B
+    assert tuple(tar_images.shape) == (B, TH, TW, 3) and tuple(ref_masks.shape) == (B, RH, RW) and geom.dtype == torch.int32
+    _lib.check(_lib.load().anysd_anydoor_prepare(_ptr(ref_images), _ptr(ref_masks), RH, RW, _ptr(tar_images), TH, TW, B, _ptr(geom),
+                                                 *(_ptr(st[k]) for k in keys), _stream()), "anydoor_prepare")
+    _count(5)
+
+
+def anydoor_sobel(ref_u8, mask_u8, st):
+    """tools/tool.py sobel (three launches): uint8 [B, 224, 224, 3] image and [B, 224, 224] mask (the uint8 it is k / 255 of)
+    -> the stage tensors img256, m256, hf256 and hf224 of ``st``."""
+    keys = ("img256", "m256", "hf256", "hf224")
+    _cuda(ref_u8, mask_u8, *(st[k] for k in keys))
+    B = ref_u8.shape[0]
+    assert tuple(ref_u8.shape) == (B, 224, 224, 3) and tuple(mask_u8.shape) == (B, 224, 224)
+    assert all(t.is_contiguous() and t.dtype == torch.uint8 for t in (ref_u8, mask_u8, *(st[k] for k in keys)))
+    _lib.check(_lib.load().anysd_anydoor_sobel(_ptr(ref_u8), _ptr(mask_u8), B, *(_ptr(st[k]) for k in keys), _stream()),
+               "anydoor_sobel")
+    _count(3)
+
+
+def anydoor_crop_back(src, tar_images, geom, out):
+    """AnyDoor's crop_back pasted into uint8 tar_images [B, H, W, 3] -> out (same shape).  src: the decoded images fp32
+    [B, 3, 512, 512] (scaled, clipped and cut in the kernel), or crop_back's own pred fp32 [B, 511, 512, 3]."""
+    _cuda(src, tar_images, geom, out)
+    B, H, W, _ = tar_images.shape
+    decoded = tuple(src.shape) == (B, 3, 512, 512)
+    assert src.dtype == torch.float32 and (decoded or tuple(src.shape) == (B, 511, 512, 3)) and src.is_contiguous()
+    assert out.dtype == tar_images.dtype == torch.uint8 and out.shape == tar_images.shape and tar_images.is_contiguous()
+    _lib.check(_lib.load().anysd_anydoor_crop_back(_ptr(src), int(decoded), _ptr(tar_images), B, H, W, _ptr(geom), _ptr(out), _stream()),
+               "anydoor_crop_back")
+    _count()
+
 # ---- training step (SURVEY.md a24): thin wrappers, same conventions as above -------------------------------------
 def q_sample(x0, noise, t, sqrt_acp, sqrt_1m_acp, out):
     _cuda(x0, noise, t, out)

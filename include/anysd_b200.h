@@ -340,6 +340,28 @@ int anysd_hed_edges_u8(const float* const* maps, const int* sizes, int ld, int N
  * low < 0, low > high and B H W > 2^31 - 1 (a label is a pixel index). */
 size_t anysd_sketch_workspace_bytes(int B, int H, int W);
 int anysd_sketch_u8(const void* img, int B, int H, int W, int low, int high, void* workspace, void* out, anysd_stream_t stream);
+/* cv2.resize(INTER_LINEAR) of uint8 images, equal to OpenCV on every byte (its exact-2x INTER_AREA branch included): src [B, H, W, C]
+ * -> dst [B, OH, OW, C].  11-bit weights, the vertical pass as OpenCV's vector code rounds it (oracle/anydoor_oracle.py resize_u8). */
+int anysd_resize_linear_u8(const void* src, int B, int H, int W, int C, void* dst, int OH, int OW, anysd_stream_t stream);
+/* AnyDoor's visual-reference request (visual_reference_tool.py process_pairs / crop_back, tools/tool.py sobel), equal to the
+ * reference.  anysd_anydoor_bbox_u8: masks uint8 [B, H, W] -> out int32 [B, 6] = (sum, first row, last row, first column, last
+ * column, largest value).  geom: int32 [B, ANYDOOR_P], the host's box geometry per pair (anyedit_b200/anydoor.py).
+ * anysd_anydoor_prepare (five launches, anysd_anydoor_sobel's three among them): ref images uint8 [B, RH, RW, 3], ref masks uint8
+ * 0/1 [B, RH, RW], tar images uint8 [B, TH, TW, 3] -> the stages ref_u8
+ * [B, 224, 224, 3], mask_u8 [B, 224, 224], img256 [B, 256, 256, 3], m256 [B, 256, 256], hf256 [B, 256, 256, 3], hf224
+ * [B, 224, 224, 3] and the model inputs ref_f32 [B, 224, 224, 3], jpg [B, 512, 512, 3], hint [B, 512, 512, 4] (fp32).
+ * anysd_anydoor_crop_back: src pasted into tar_img uint8 [B, H, W, 3] -> out; src is the decoded images fp32 [B, 3, 512, 512]
+ * (decoded = 1: * 127.5 + 127.5, clipped, first row dropped here) or crop_back's pred fp32 [B, 511, 512, 3] (decoded = 0). */
+#define ANYDOOR_P 18
+int anysd_anydoor_bbox_u8(const void* masks, int B, int H, int W, void* out, anysd_stream_t stream);
+int anysd_anydoor_prepare(const void* ref_img, const void* ref_mask, int RH, int RW, const void* tar_img, int TH, int TW, int B, const void* geom,
+                          void* ref_u8, void* mask_u8, void* img256, void* m256, void* hf256, void* hf224, void* ref_f32, void* jpg,
+                          void* hint, anysd_stream_t stream);
+/* tools/tool.py sobel of the 224 x 224 stage (ref_u8, mask_u8 as above) -> img256, m256, hf256, hf224; three launches. */
+int anysd_anydoor_sobel(const void* ref_u8, const void* mask_u8, int B, void* img256, void* m256, void* hf256, void* hf224,
+                        anysd_stream_t stream);
+int anysd_anydoor_crop_back(const void* src, int decoded, const void* tar_img, int B, int H, int W, const void* geom, void* out,
+                            anysd_stream_t stream);
 
 /* ==== training step (SURVEY.md a24; train.py:629-710) =====================================================
  * The reference back-propagates mse_loss(MoE(...), noise) through the frozen UNet with torch autograd
