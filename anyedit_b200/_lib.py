@@ -81,6 +81,7 @@ SIGNATURES = {
     "anysd_nhwc_to_nchw": (_I, [_VP, _I, _I, _VP, _I, _I, _I, _I, _I, _VP]),
     "anysd_concat_channels_f16": (_I, [_VP, _I, _VP, _I, _VP, _LL, _VP]),
     "anysd_cast_f32_to_f16": (_I, [_VP, _VP, _LL, _VP]),
+    "anysd_image_to_u8": (_I, [_VP, _VP, _I, _I, _I, _I, _VP]),
     "anysd_timestep_embedding_f16": (_I, [_VP, _I, _VP, _I, _I, _F, _VP]),
     "anysd_emb_finalize": (_I, [_VP, _VP, _VP, _I, _VP, _VP, _I, _I, _VP]),
     "anysd_router_gate_f32": (_I, [_VP, _VP, _I, _VP, _VP, _VP, _I, _I, _I, _I, _VP]),
@@ -95,6 +96,7 @@ SIGNATURES = {
     "anysd_xattn_block_f16": (_I, [_VP] * 8 + [_I] + [_VP] * 7 + [_I] * 8 + [_F, _VP]),
     "anysd_groupnorm_apply_nhwc_f16": (_I, [_VP, _I, _VP, _I, _VP, _I, _VP, _VP, _VP, _I, _I, _I, _F, _I, _VP, _SZ, _VP]),
     "anysd_attention_f16": (_I, [C.POINTER(AttnParams), _VP]),
+    "anysd_attention_kvmap_f16": (_I, [C.POINTER(AttnParams), _VP, _VP]),
     "anysd_cfg_ddim_step_f32": (_I, [_VP, _VP, _VP, _VP, _F, _I, _I, _VP, _VP, _LL, _I, _VP]),
     "anysd_cfg3_ddim_step_f32": (_I, [_VP, _VP, _VP, _VP, _F, _F, _VP, _VP, _LL, _I, _VP]),
     "anysd_cfg_plms_step_f32": (_I, [_VP, _VP, _VP, _F, _I, _VP, _VP, _VP, _LL, _I, _VP]),

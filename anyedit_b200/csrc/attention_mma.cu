@@ -11,7 +11,7 @@
 
 namespace anysd {
 
-int launch_attention_wg(const anysd_attn_params* q, cudaStream_t st);
+int launch_attention_wg(const anysd_attn_params* q, const int* kv_batch, cudaStream_t st);
 bool attention_wg_supported(const anysd_attn_params* q);
 
 constexpr int ATT_BQ = 64, ATT_BKV = 64, ATT_THREADS = 128;
@@ -24,6 +24,7 @@ struct AttnArgs {
     float scale_log2;
     const float* gate;
     int gate_stride, accumulate;
+    const int* kv_batch;                      // optional [B]: query batch b reads the K/V of batch kv_batch[b]
 };
 
 __device__ __forceinline__ float ex2(float x) {
@@ -46,8 +47,9 @@ __global__ void __launch_bounds__(ATT_THREADS) attention_mma_kernel(const AttnAr
     const int b = blockIdx.z, h = blockIdx.y, q0 = blockIdx.x * ATT_BQ;
     const int dch = p.d / 8;                  // real chunks per row
     const __half* qg = p.q + (size_t)b * p.qbs + (size_t)h * p.hs;
-    const __half* kg = p.k + (size_t)b * p.kbs + (size_t)h * p.hs;
-    const __half* vg = p.v + (size_t)b * p.vbs + (size_t)h * p.hs;
+    const int kvb = p.kv_batch ? __ldg(p.kv_batch + b) : b;
+    const __half* kg = p.k + (size_t)kvb * p.kbs + (size_t)h * p.hs;
+    const __half* vg = p.v + (size_t)kvb * p.vbs + (size_t)h * p.hs;
 
     auto load_tile = [&](const __half* g, int ld, int row0, int nrows, __half* s) {
         for (int i = tid; i < ATT_BKV * CH; i += ATT_THREADS) {
@@ -208,7 +210,7 @@ static int launch_attn(const AttnArgs& a, int B, int heads, cudaStream_t st) {
     return check_launch("attention (mma.sync)");
 }
 
-int launch_attention_mma(const anysd_attn_params* q, cudaStream_t st) {
+int launch_attention_mma(const anysd_attn_params* q, const int* kv_batch, cudaStream_t st) {
     AttnArgs a;
     a.q = (const __half*)q->q; a.k = (const __half*)q->k; a.v = (const __half*)q->v; a.out = (__half*)q->out;
     a.qbs = q->q_batch_stride; a.kbs = q->k_batch_stride; a.vbs = q->v_batch_stride; a.obs = q->o_batch_stride;
@@ -217,6 +219,7 @@ int launch_attention_mma(const anysd_attn_params* q, cudaStream_t st) {
     a.hs = q->head_stride > 0 ? q->head_stride : q->d;
     a.scale_log2 = q->scale * 1.4426950408889634f;
     a.gate = q->gate; a.gate_stride = q->gate_stride; a.accumulate = q->accumulate;
+    a.kv_batch = kv_batch;
     const int dp = (q->d + 15) / 16 * 16;
     switch (dp) {
         case 16: return launch_attn<16>(a, q->B, q->heads, st);
@@ -237,7 +240,7 @@ int launch_attention_mma(const anysd_attn_params* q, cudaStream_t st) {
 
 using namespace anysd;
 
-extern "C" int anysd_attention_f16(const anysd_attn_params* p, anysd_stream_t stream) {
+static int attention_run(const anysd_attn_params* p, const int* kv_batch, anysd_stream_t stream) {
     ANYSD_REQUIRE(p != nullptr, ANYSD_EINVAL, "attention: null params");
     ANYSD_REQUIRE(p->q && p->k && p->v && p->out, ANYSD_EINVAL, "attention: null pointer");
     ANYSD_REQUIRE(p->B > 0 && p->heads > 0 && p->n_q > 0 && p->n_kv > 0, ANYSD_EINVAL, "attention: bad sizes");
@@ -253,12 +256,21 @@ extern "C" int anysd_attention_f16(const anysd_attn_params* p, anysd_stream_t st
     ANYSD_REQUIRE(p->heads <= 65535 && p->B <= 65535, ANYSD_EINVAL, "attention: grid too large");
     ANYSD_REQUIRE(p->head_stride == 0 || (p->head_stride >= p->d && p->head_stride % 8 == 0), ANYSD_EINVAL,
                   "attention: head_stride must be 0 or a multiple of 8 >= d");
+    ANYSD_REQUIRE(((uintptr_t)kv_batch % 4) == 0, ANYSD_EINVAL, "attention: kv_batch must be 4-byte aligned");
     // wgmma kernel whenever its layout constraints hold; ANYSD_ATTN=mma|wgmma is a test/debug switch.
     static const char* force = getenv("ANYSD_ATTN");
     const bool want_wg = !force || !strcmp(force, "wgmma");
-    if (want_wg && attention_wg_supported(p)) return launch_attention_wg(p, (cudaStream_t)stream);
+    if (want_wg && attention_wg_supported(p)) return launch_attention_wg(p, kv_batch, (cudaStream_t)stream);
     ANYSD_REQUIRE(p->lse == nullptr, ANYSD_EUNSUPPORTED, "attention: the log-sum-exp output needs the wgmma kernel");
     ANYSD_REQUIRE(!p->aux_cols, ANYSD_EUNSUPPORTED,
                   "attention: aux_cols needs the wgmma kernel (d %% 16 == 8, head_stride >= d + 8, stacked batches)");
-    return launch_attention_mma(p, (cudaStream_t)stream);
+    return launch_attention_mma(p, kv_batch, (cudaStream_t)stream);
+}
+
+extern "C" int anysd_attention_f16(const anysd_attn_params* p, anysd_stream_t stream) {
+    return attention_run(p, nullptr, stream);
+}
+
+extern "C" int anysd_attention_kvmap_f16(const anysd_attn_params* p, const int* kv_batch, anysd_stream_t stream) {
+    return attention_run(p, kv_batch, stream);
 }

@@ -38,6 +38,7 @@ struct AwArgs {
     const float* gate;
     int gate_stride, accumulate;
     float* lse;                        // optional [B, heads, n_q]: base-2 log-sum-exp of every score row
+    const int* kv_batch;               // optional [B]: query batch b reads the K/V rows of batch kv_batch[b]
 };
 
 __device__ __forceinline__ void aw_init(uint32_t bar, uint32_t count) {
@@ -124,6 +125,7 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
         asm volatile("setmaxnreg.dec.sync.aligned.u32 24;" ::: "memory");
         if (warp == 0 && lane == 0) {
             const int col0 = h * p.hs;
+            const int kv_row0 = (p.kv_batch ? __ldg(p.kv_batch + b) : b) * p.n_kv;
             aw_expect_tx(BAR(0), NA * AW_ATOM);
             for (int a = 0; a < NA; ++a) aw_tma_2d(base + a * AW_ATOM, &tmQ, BAR(0), col0 + a * 64, b * p.n_q + q0);
             for (int j = 0; j < nt; ++j) {
@@ -131,8 +133,8 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
                 aw_wait(BAR(1 + ST + s), (((uint32_t)j / ST) & 1) ^ 1);
                 aw_expect_tx(BAR(1 + s), Cfg::STAGE_BYTES);
                 const uint32_t kb = base + kv_off + s * Cfg::STAGE_BYTES, vb = kb + NA * KV_ATOM;
-                for (int a = 0; a < NA; ++a) aw_tma_2d(kb + a * KV_ATOM, &tmK, BAR(1 + s), col0 + a * 64, b * p.n_kv + j * BKV);
-                for (int a = 0; a < NA; ++a) aw_tma_2d(vb + a * KV_ATOM, &tmV, BAR(1 + s), col0 + a * 64, b * p.n_kv + j * BKV);
+                for (int a = 0; a < NA; ++a) aw_tma_2d(kb + a * KV_ATOM, &tmK, BAR(1 + s), col0 + a * 64, kv_row0 + j * BKV);
+                for (int a = 0; a < NA; ++a) aw_tma_2d(vb + a * KV_ATOM, &tmV, BAR(1 + s), col0 + a * 64, kv_row0 + j * BKV);
             }
         }
         return;
@@ -370,7 +372,7 @@ static int aw_launch(const anysd_attn_params* q, const AwArgs& a, cudaStream_t s
     return check_launch("attention (wgmma)");
 }
 
-int launch_attention_wg(const anysd_attn_params* q, cudaStream_t st) {
+int launch_attention_wg(const anysd_attn_params* q, const int* kv_batch, cudaStream_t st) {
     AwArgs a;
     a.out = (__half*)q->out;
     a.obs = q->o_batch_stride;
@@ -380,6 +382,7 @@ int launch_attention_wg(const anysd_attn_params* q, cudaStream_t st) {
     a.scale_log2 = q->aux_cols ? 1.0f : q->scale * 1.4426950408889634f;
     a.gate = q->gate; a.gate_stride = q->gate_stride; a.accumulate = q->accumulate;
     a.lse = q->lse;
+    a.kv_batch = kv_batch;
     switch ((q->d + 15) / 16 * 16) {
         case 16: return aw_launch<16>(q, a, st);
         case 32: return aw_launch<32>(q, a, st);

@@ -56,6 +56,20 @@ __global__ void concat_kernel(const uint4* __restrict__ a, int va, const uint4* 
     }
 }
 
+// decoded image (NCHW fp32 in [-1, 1]) -> NHWC uint8, as diffusers post-processes it: round(clamp(x / 2 + 1/2, 0, 1) * 255),
+// each step rounded to fp32 (no FMA) and the last one half to even, like numpy's round
+__global__ void image_to_u8_kernel(const float* __restrict__ src, unsigned char* __restrict__ dst, int C, int HW, long long n) {
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+        const long long px = i / C;
+        const int c = (int)(i - px * C);
+        const long long img = px / HW;
+        const int hw = (int)(px - img * HW);
+        float t = __fadd_rn(__fmul_rn(src[(img * C + c) * HW + hw], 0.5f), 0.5f);
+        t = fminf(fmaxf(t, 0.f), 1.f);
+        dst[i] = (unsigned char)rintf(__fmul_rn(t, 255.f));
+    }
+}
+
 __global__ void cast_kernel(const float* __restrict__ src, __half* __restrict__ dst, long long n) {
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n;
          i += (long long)gridDim.x * blockDim.x)
@@ -347,6 +361,15 @@ int anysd_cast_f32_to_f16(const float* src, void* dst, long long n, anysd_stream
     if (grid > sm_count() * 16) grid = sm_count() * 16;
     cast_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(src, (__half*)dst, n);
     return check_launch("cast");
+}
+
+int anysd_image_to_u8(const float* src, void* dst, int N, int C, int H, int W, anysd_stream_t stream) {
+    ANYSD_REQUIRE(src && dst && N > 0 && C > 0 && H > 0 && W > 0, ANYSD_EINVAL, "image_to_u8: bad args");
+    const long long n = (long long)N * C * H * W;
+    int grid = (int)((n + 255) / 256);
+    if (grid > sm_count() * 16) grid = sm_count() * 16;
+    image_to_u8_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(src, (unsigned char*)dst, C, H * W, n);
+    return check_launch("image_to_u8");
 }
 
 int anysd_timestep_embedding_f16(const void* t, int t_dtype, void* out, int N, int dim, float max_period,

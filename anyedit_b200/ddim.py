@@ -77,7 +77,8 @@ class DDIMSampler(object):
         gk = getattr(self.model, "graph_key", None)      # changes whenever the model's packed weights change
         key = (b, tuple(shape), bool(use_cfg), bool(graph), str(device), _tree_sig(cond),
                _tree_sig(uncond) if use_cfg else None, gk() if callable(gk) else gk,
-               None if img_cond is None else (_tree_sig(img_cond), float(img_scale)), update)
+               None if img_cond is None else (_tree_sig(img_cond), float(img_scale)), update,
+               _editor_of(self.model) is not None)
         st = self._graphs.get(key)
         if st is None:
             if len(self._graphs) >= 4:
@@ -221,11 +222,21 @@ class DDIMSampler(object):
             assert unconditional_conditioning is not None, "three-way guidance needs the unconditional conditioning too"
             use_cfg = True
         sigma_nonzero = bool(np.any(sigmas_used[:total_steps] != 0))
+        editor = _editor_of(self.model)
+        if editor is not None and three:
+            raise NotImplementedError("three-way InstructPix2Pix guidance with an attention editor attached (anyedit_b200.masactrl)")
 
         stepper = self._get_stepper(cond, unconditional_conditioning, use_cfg, b, tuple(shape), device,
                                     graph=self.use_cuda_graph and ucg_schedule is None and hooks is None,
                                     img_cond=image_conditioning if three else None, img_scale=image_guidance_scale if three else None)
         stepper.hooks = hooks
+        kv_steps = None
+        if editor is not None:
+            # the editor's K/V map of every step of this run, [S, blocks, N], uploaded once; row i is copied into the
+            # stepper's static buffer before step i (eager or replayed), as ddim_coef[index] is into coef_buf
+            from .masactrl import kv_table
+            kv_steps = torch.from_numpy(kv_table(editor, stepper.kv_buf.shape[0], stepper.kv_buf.shape[1], editor.cur_step,
+                                                 len(time_range))).to(device)
         for i, step in enumerate(time_range):
             index = total_steps - i - 1
             if mask is not None:
@@ -243,8 +254,12 @@ class DDIMSampler(object):
                     noise = torch.nn.functional.dropout(noise, p=noise_dropout)
                 if not sigma_nonzero:
                     noise = None
+            if kv_steps is not None:
+                stepper.kv_buf.copy_(kv_steps[i])
             img, pred_x0 = stepper.step(img, index, int(step), scale, noise,
                                         coef=None if coef_table is None else coef_table[index])
+            if editor is not None:
+                editor.cur_step += 1                      # one UNet forward per step, as the reference's editor counts
             if callback:
                 callback(i)
             if img_callback:
@@ -272,6 +287,7 @@ class DDIMSampler(object):
                       temperature=1., noise_dropout=0., score_corrector=None, corrector_kwargs=None,
                       unconditional_guidance_scale=1., unconditional_conditioning=None, dynamic_threshold=None):
         """One step (ddim.py:181-251); used by ``decode`` and by callers that drive the loop themselves."""
+        _refuse_editor(self.model, "DDIMSampler.p_sample_ddim")
         hooks = self._step_hooks(score_corrector, corrector_kwargs, quantize_denoised, c, None)
         if dynamic_threshold is not None:
             raise NotImplementedError()
@@ -298,6 +314,7 @@ class DDIMSampler(object):
         """DDIM inversion (ddim.py:253-299).  Same arithmetic and the same quirk as the reference (the model is
         called with t = loop index i, not with the DDIM timestep); the per-step update
         x_next = sqrt(a_next/a) x + sqrt(a_next) (sqrt(1/a_next - 1) - sqrt(1/a - 1)) eps runs in the fused kernel."""
+        _refuse_editor(self.model, "DDIMSampler.encode")
         if use_original_steps:
             raise NotImplementedError("use_original_steps is not on the AnySD path")
         num_reference_steps = self.ddim_timesteps.shape[0]
@@ -346,6 +363,7 @@ class DDIMSampler(object):
     @torch.no_grad()
     def decode(self, x_latent, cond, t_start, unconditional_guidance_scale=1.0, unconditional_conditioning=None,
                use_original_steps=False, callback=None):
+        _refuse_editor(self.model, "DDIMSampler.decode")
         if use_original_steps:
             raise NotImplementedError("use_original_steps is not on the AnySD path")
         timesteps = self.ddim_timesteps[:t_start]
@@ -411,6 +429,18 @@ def _find_unet(model):
     from .unet import UNetModel
     m = getattr(getattr(model, "model", None), "diffusion_model", None)
     return m if isinstance(m, UNetModel) else None
+
+
+def _editor_of(model):
+    """The attention editor registered on the model's anyedit_b200 UNet (anyedit_b200.masactrl), or None."""
+    u = _find_unet(model)
+    return None if u is None else getattr(u, "_editor", None)
+
+
+def _refuse_editor(model, what):
+    if _editor_of(model) is not None:
+        raise NotImplementedError(f"{what} with an attention editor attached (anyedit_b200.masactrl): only DDIMSampler.sample "
+                                  "runs the edit; detach it with regiter_attention_editor_ldm(model, None)")
 
 
 def _tree_sig(c):
@@ -486,6 +516,14 @@ class _Stepper:
         self.kv = {"mode": "fill", "bufs": []} if self.unet is not None and os.environ.get("ANYSD_CTX_KV", "1")[:1] != "0" else None
         self.kv_dirty = True
         self.hooks = None                            # (score_corrector, its kwargs, quantize_denoised, cond): see DDIMSampler._step_hooks
+        # attention editor (anyedit_b200.masactrl): the K/V map of the current step, [blocks, N] int32, in a static buffer
+        # the captured graph reads (identity until the sampler copies a step's row in)
+        self.kv_buf = None
+        if self.unet is not None and getattr(self.unet, "_editor", None) is not None:
+            if update != "ddim":
+                raise NotImplementedError(f"the {'PLMS' if update == 'plms' else 'DPM-Solver'} sampler with an attention editor "
+                                          "attached (anyedit_b200.masactrl): only DDIMSampler.sample runs the edit")
+            self.kv_buf = torch.arange(nb, dtype=torch.int32, device=device).repeat(self.unet.num_transformer_blocks(), 1)
 
     def _hooked_update(self, eps, scale, noise):
         """ddim.py:194-251 as the reference writes it (separate fp32 tensor ops, in its order), with the hooks in place."""
@@ -535,6 +573,8 @@ class _Stepper:
             self.unet._shared_halves = True              # x, c_concat and t of the two halves are identical
         if self.kv is not None:
             self.unet._ctx_kv = self.kv
+        if self.kv_buf is not None:
+            self.unet._kv_rows = self.kv_buf
         try:
             eps = self.s.model.apply_model(self.x_in, self.t_buf, self.c_in)
         finally:
@@ -542,6 +582,8 @@ class _Stepper:
                 self.unet._shared_halves = False
             if self.kv is not None:
                 self.unet._ctx_kv = None
+            if self.kv_buf is not None:
+                self.unet._kv_rows = None
         eps = eps.float().contiguous()
         self.last_eps = eps                              # the model output of the latest step (parity tests / bench read it)
         if self.hooks is not None:

@@ -375,10 +375,13 @@ def conv3x3(x, W, out, bias=None, rowadd=None, residual=None, stride=1, upsample
 
 
 def attention(q, k, v, out, B, heads, n_q, n_kv, d, ld_q, ld_k, ld_v, ld_o, q_bs=None, k_bs=None, v_bs=None,
-              o_bs=None, scale=None, gate=None, gate_stride=1, accumulate=False, head_stride=0, aux_cols=False, lse=None):
+              o_bs=None, scale=None, gate=None, gate_stride=1, accumulate=False, head_stride=0, aux_cols=False, lse=None,
+              kv_batch=None):
     """softmax(q k^T * scale) v per (batch, head); q/k/v may be column slices of fused projections.
-    ``lse`` (fp32 [B, heads, n_q]): also store the base-2 log-sum-exp of every score row (for the backward)."""
-    _cuda(q, k, v, out)
+    ``lse`` (fp32 [B, heads, n_q]): also store the base-2 log-sum-exp of every score row (for the backward).
+    ``kv_batch`` (int32 [B] on the device, entries in [0, B)): query batch b attends to the K/V of batch kv_batch[b]
+    (anysd_attention_kvmap_f16); None launches anysd_attention_f16."""
+    _cuda(q, k, v, out, kv_batch)
     p = AttnParams()
     p.q, p.k, p.v, p.out = q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr()
     p.q_batch_stride = q_bs if q_bs is not None else n_q * ld_q
@@ -396,8 +399,24 @@ def attention(q, k, v, out, B, heads, n_q, n_kv, d, ld_q, ld_k, ld_v, ld_o, q_bs
     if lse is not None:
         assert lse.dtype == torch.float32 and lse.is_contiguous() and lse.numel() == B * heads * n_q
         p.lse = lse.data_ptr()
-    with _Traced("attention", 4.0 * B * heads * n_q * n_kv * d, f"B={B} h={heads} nq={n_q} nkv={n_kv} d={d}"):
-        _lib.check(_lib.load().anysd_attention_f16(C.byref(p), _stream()), "attention")
+    if kv_batch is not None:
+        assert kv_batch.dtype == torch.int32 and kv_batch.is_contiguous() and kv_batch.numel() == B
+        with _Traced("attention", 4.0 * B * heads * n_q * n_kv * d, f"B={B} h={heads} nq={n_q} nkv={n_kv} d={d} kvmap"):
+            _lib.check(_lib.load().anysd_attention_kvmap_f16(C.byref(p), _ptr(kv_batch), _stream()), "attention_kvmap")
+    else:
+        with _Traced("attention", 4.0 * B * heads * n_q * n_kv * d, f"B={B} h={heads} nq={n_q} nkv={n_kv} d={d}"):
+            _lib.check(_lib.load().anysd_attention_f16(C.byref(p), _stream()), "attention")
+    _count()
+
+
+def image_to_u8(images, out):
+    """Decoded images fp32 NCHW [N, C, H, W] in [-1, 1] -> out uint8 NHWC [N, H, W, C] = round(clamp(x / 2 + 1/2, 0, 1) * 255)
+    (diffusers' post-processing, rounding half to even)."""
+    _cuda(images, out)
+    N, Cc, H, W = images.shape
+    assert images.dtype == torch.float32 and images.is_contiguous()
+    assert out.dtype == torch.uint8 and out.is_contiguous() and tuple(out.shape) == (N, H, W, Cc)
+    _lib.check(_lib.load().anysd_image_to_u8(_ptr(images), _ptr(out), N, Cc, H, W, _stream()), "image_to_u8")
     _count()
 
 

@@ -344,6 +344,8 @@ class UNetModel(nn.Module):
         self._pack = None
         self._pack_key = None
         self._epoch = 0                  # bumped by invalidate(): part of the pack key and of LatentDenoiser.graph_key
+        self._editor = None              # attention editor (anyedit_b200.masactrl.regiter_attention_editor_ldm)
+        self._kv_rows = None             # the sampler's static K/V map buffer for the editor, set around each step
 
     # the reference's no-op stubs (openaimodel.py:738-752)
     def convert_to_fp16(self):
@@ -521,7 +523,7 @@ class UNetModel(nn.Module):
         emb_all = self._embeddings(P, N, timesteps, y, anysd, dev)
         ctx16 = self._context16(context, N, dev)
         st = {"N": N, "ws": ws, "emb_all": emb_all, "ctx": ctx16, "anysd": anysd, "layer": 0, "xl": 0,
-              "kvc": getattr(self, "_ctx_kv", None)}
+              "kvc": getattr(self, "_ctx_kv", None), "kvmap": self._kv_rows_for_forward(N, dev), "blk": 0}
 
         # -- input conv --
         # Shared CFG halves (set by the DDIM stepper when x, c_concat, t and y of the uncond / cond halves are
@@ -572,6 +574,28 @@ class UNetModel(nn.Module):
         out = torch.empty(N, self.out_channels, Hh, Ww, dtype=out_dtype, device=dev)
         ops.nhwc_to_nchw(o, out)
         return out.to(x.dtype)
+
+    def num_transformer_blocks(self):
+        """BasicTransformerBlocks of the UNet (16 for SD-1.5); the reference's attention editors count 2 per block."""
+        return sum(isinstance(m, _TransformerBlock) for m in self.modules())
+
+    def _kv_rows_for_forward(self, N, dev):
+        """The self-attention K/V batch map of this forward, int32 [blocks, N] on the device (row i for the i-th transformer
+        block in forward order), or None when no attention editor is registered (anyedit_b200.masactrl).  A sampler that
+        drives the editor itself hands a static buffer over (``_kv_rows``, refreshed before every step); otherwise the
+        editor's active set for its ``cur_step`` is read here and ``cur_step`` advances by one, as the reference's editor
+        counts one step per UNet forward (masactrl_utils.py:22-31)."""
+        rows = getattr(self, "_kv_rows", None)
+        if rows is not None:
+            assert tuple(rows.shape) == (self.num_transformer_blocks(), N), "K/V map does not fit this forward"
+            return rows
+        editor = getattr(self, "_editor", None)
+        if editor is None:
+            return None
+        from .masactrl import kv_table
+        table = kv_table(editor, self.num_transformer_blocks(), N, editor.cur_step, 1)
+        editor.cur_step += 1
+        return torch.from_numpy(table[0]).to(dev)
 
     def _embeddings(self, P, N, timesteps, y, anysd, dev):
         """time / class / task embedding (openaimodel.py:767-772) -> the stacked ResBlock ``emb_layers`` rows [N, sum Cout] fp32."""
@@ -666,11 +690,13 @@ class UNetModel(nn.Module):
         out._gn = ops.conv3x3(b, d["c2_w"], out.view(-1, cout), bias=d["c2_b"], residual=res, stats=True)
         return out
 
-    def _attn(self, ad, xq, ctx, N, n_q, st, self_attn, residual, out, expert=False, q_pre=None, ln=None, out_stats=False):
+    def _attn(self, ad, xq, ctx, N, n_q, st, self_attn, residual, out, expert=False, q_pre=None, ln=None, out_stats=False,
+              kv_batch=None):
         """CrossAttention.forward (attention.py:163-194) + residual add of the caller (:272-273).
         ``q_pre``: the query projection computed by the caller (shared CFG halves), ``xq`` is then unused.
         ``ln`` = (row moments of xq, folded pack): xq is the UN-normalised input of the block's LayerNorm, which is folded into
-        the query (/ fused q|k|v) projection; ``out_stats``: the output projection leaves ``out._ln`` for the next LayerNorm."""
+        the query (/ fused q|k|v) projection; ``out_stats``: the output projection leaves ``out._ln`` for the next LayerNorm.
+        ``kv_batch``: the self-attention's K/V batch map (int32 [N] on the device, an attention editor's), or None."""
         C = ad["heads"] * ad["d"]
         hs = ad["hs"]
         Cp = ad["heads"] * hs                     # projection width with padded heads (== C unless d % 16 != 0)
@@ -683,7 +709,7 @@ class UNetModel(nn.Module):
             else:
                 ops.gemm(xq, ad["qkv_w"], qkv, bias=ad["qkv_b"])
             ops.attention(qkv, qkv[:, Cp:], qkv[:, 2 * Cp:], a, N, ad["heads"], n_q, n_q, ad["d"],
-                          3 * Cp, 3 * Cp, 3 * Cp, C, head_stride=hs, aux_cols=ad["aux"])
+                          3 * Cp, 3 * Cp, 3 * Cp, C, head_stride=hs, aux_cols=ad["aux"], kv_batch=kv_batch)
         else:
             L = ctx.shape[1]
             if q_pre is not None:
@@ -789,6 +815,12 @@ class UNetModel(nn.Module):
         ops.gemm(g.view(M, C), d["pin_w"], t, bias=d["pin_b"], row_stats=t._ln if fold0 else None)
         for i, b in enumerate(d["blocks"]):
             ctx = st["ctx"][i] if i < len(st["ctx"]) else st["ctx"][-1]
+            kvb = None
+            if st.get("kvmap") is not None:
+                # this block's row of the editor's K/V map; on shared CFG halves the first half of it, which is exact
+                # because every map satisfies map[b + N/2] = map[b] + N/2 (masactrl.kv_batch_map)
+                kvb = st["kvmap"][st["blk"]][:N] if b["self"] else None
+                st["blk"] += 1
             if share and not b["self"]:
                 # disable_self_attn: attn1 already attends to the context, which differs between the CFG halves --
                 # nothing more can be shared, widen to the full batch here
@@ -799,7 +831,7 @@ class UNetModel(nn.Module):
                 # 320 channels: attn1's output projection through norm3 in one launch, then the fused feed-forward
                 ln = torch.empty_like(t)
                 ops.layernorm(t, b["ln1_w"], b["ln1_b"], ln)
-                a1 = self._attn(b["attn1"], ln, None, N, n, st, True, t, None)
+                a1 = self._attn(b["attn1"], ln, None, N, n, st, True, t, None, kv_batch=kvb)
                 if share:
                     # shared CFG halves: widen before attn1's output projection (identical halves, bit-identical result)
                     a1, t, h = self._dup_rows(a1), self._dup_rows(t), self._dup_rows(h)
@@ -819,13 +851,14 @@ class UNetModel(nn.Module):
                 # producer of t / t2 / t3 has left per-row moments, the consumer takes the un-normalised rows
                 fb = self._ln_folded(b)
                 t2 = torch.empty_like(t)
-                self._attn(b["attn1"], t, None if b["self"] else ctx, N, n, st, b["self"], t, t2, ln=(t._ln, fb["a1"]), out_stats=True)
+                self._attn(b["attn1"], t, None if b["self"] else ctx, N, n, st, b["self"], t, t2, ln=(t._ln, fb["a1"]), out_stats=True,
+                           kv_batch=kvb)
             else:
                 ln = torch.empty_like(t)
                 ops.layernorm(t, b["ln1_w"], b["ln1_b"], ln)
                 t2 = torch.empty_like(t)
                 if b["self"]:
-                    self._attn(b["attn1"], ln, None, N, n, st, True, t, t2)
+                    self._attn(b["attn1"], ln, None, N, n, st, True, t, t2, kv_batch=kvb)
                 else:
                     self._attn(b["attn1"], ln, ctx, N, n, st, False, t, t2)
                 ln2 = torch.empty_like(t)

@@ -57,6 +57,9 @@ int anysd_nhwc_to_nchw(const void* src, int src_dtype, int src_C, void* dst, int
 int anysd_concat_channels_f16(const void* a, int Ca, const void* b, int Cb, void* dst, long long rows,
                               anysd_stream_t stream);
 int anysd_cast_f32_to_f16(const float* src, void* dst, long long n, anysd_stream_t stream);
+/* Decoded images, fp32 NCHW [N, C, H, W] in [-1, 1] -> uint8 NHWC [N, H, W, C] as diffusers post-processes them
+ * (image_processor / numpy_to_pil): round(clamp(x / 2 + 1/2, 0, 1) * 255) in fp32, rounding half to even. */
+int anysd_image_to_u8(const float* src, void* dst, int N, int C, int H, int W, anysd_stream_t stream);
 
 /* ---- time / task embedding ---------------------------------------------------------------
  * timestep_embedding (ldm/modules/diffusionmodules/util.py:154-174): cos half first. */
@@ -222,6 +225,11 @@ typedef struct {
                                to recompute the probabilities without its own pass over K (train.py:694-709 backward). */
 } anysd_attn_params;
 int anysd_attention_f16(const anysd_attn_params* p, anysd_stream_t stream);
+/* The same attention with a K/V batch map (MasaCtrl's mutual self-attention, masactrl.py:41-72): query batch b attends to
+ * the K/V rows of batch kv_batch[b].  kv_batch: device int32 [B], every entry in [0, B) (not checked: the map is read on
+ * the device); NULL is exactly anysd_attention_f16.  Both kernels honour it (ANYSD_ATTN=mma too), with aux_cols, head_stride,
+ * gate and lse unchanged. */
+int anysd_attention_kvmap_f16(const anysd_attn_params* p, const int* kv_batch, anysd_stream_t stream);
 
 /* ---- sampler step ------------------------------------------------------------------------
  * DDIMSampler.p_sample_ddim (ldm/models/diffusion/ddim.py:211-212, 228-250), eps-parameterisation:
