@@ -8,6 +8,9 @@ before the denoising loop.
   ``CLIPVisionModelWithProjection`` the CLIP-H vision tower of train.py:688-691 (``image_encoder(..., output_hidden_states=True)
                                     .hidden_states[-2]``): patch embedding as one contraction, class token, pre-LN, 32 layers
                                     (GELU), ``vision_model.*`` / ``visual_projection`` keys.
+  ``CLIPModel``                     ``transformers.CLIPModel`` (both towers, both projection heads, ``logit_scale``): the CLIP-H
+                                    scorer of AnyEdit_Collection/filter_tool/utils.py; ``openai_clip_to_transformers`` maps
+                                    OpenAI's ``clip.load`` layout (the ViT-B/32 of the directional score) onto it.
   ``Resampler``                     AnyEdit_Collection/other_modules/ip_adapter/resampler.py:81-147 (perceiver attention of 16
                                     latent queries over [image tokens ; latents], FeedForward, proj_out + LayerNorm).
   ``ImageProjModel``                ip_adapter/ip_adapter.py:28-46.
@@ -154,42 +157,60 @@ class _TextTransformer(nn.Module):
         self.final_layer_norm = _Param((c.hidden_size,), kind="norm")
 
 
+def _text_pack(t, dev):
+    return {"tok": _h(t.embeddings.token_embedding.weight, dev), "pos": _h(t.embeddings.position_embedding.weight, dev),
+            "layers": _pack_layers(t.encoder.layers, dev),
+            "final": (_f(t.final_layer_norm.weight, dev), _f(t.final_layer_norm.bias, dev))}
+
+
+def _text_forward(P, c, input_ids, keep_hidden=False):
+    """The text tower -> (final LayerNorm fp16 [B * n, D], end-of-text positions [B], ids, hidden states)."""
+    ids = input_ids.to(device=P["tok"].device, dtype=torch.int64).contiguous()
+    B, n = ids.shape
+    h = torch.empty(B * n, c.hidden_size, dtype=torch.float16, device=ids.device)
+    ops.embed_tokens(ids, P["tok"], P["pos"], h)
+    h, hidden = _run_layers(P["layers"], h, B, n, c.num_attention_heads, _ACT[c.hidden_act], c.layer_norm_eps, causal=True,
+                            keep_hidden=keep_hidden)
+    last = torch.empty_like(h)
+    ops.layernorm(h, P["final"][0], P["final"][1], last, c.layer_norm_eps)
+    # pooled = the features at the end-of-text token (modeling_clip.py: argmax of the ids for the legacy eos id 2)
+    if c.eos_token_id == 2:
+        pos = ids.argmax(dim=-1)
+    else:
+        pos = (ids == c.eos_token_id).int().argmax(dim=-1)
+    return last, pos, ids, hidden
+
+
+_TEXT_DEFAULTS = dict(vocab_size=49408, hidden_size=768, intermediate_size=3072, num_hidden_layers=12, num_attention_heads=12,
+                      max_position_embeddings=77, hidden_act="quick_gelu", layer_norm_eps=1e-5, eos_token_id=2)
+_VISION_DEFAULTS = dict(hidden_size=1280, intermediate_size=5120, num_hidden_layers=32, num_attention_heads=16, image_size=224,
+                        patch_size=14, num_channels=3, projection_dim=1024, hidden_act="gelu", layer_norm_eps=1e-5)
+
+
+def _check_act(c):
+    if _ACT.get(c.hidden_act) is None:
+        raise NotImplementedError(f"hidden_act={c.hidden_act!r}: CLIP uses quick_gelu or gelu")
+    return c
+
+
 class CLIPTextModel(_Packable):
     """``transformers.CLIPTextModel`` (modeling_clip.py): ``forward(input_ids, output_hidden_states=False)`` ->
     namespace(last_hidden_state, pooler_output, hidden_states)."""
 
     def __init__(self, config):
         super().__init__()
-        self.config = c = _cfg(config, vocab_size=49408, hidden_size=768, intermediate_size=3072, num_hidden_layers=12,
-                               num_attention_heads=12, max_position_embeddings=77, hidden_act="quick_gelu", layer_norm_eps=1e-5,
-                               eos_token_id=2)
-        if _ACT.get(c.hidden_act) is None:
-            raise NotImplementedError(f"hidden_act={c.hidden_act!r}: CLIP uses quick_gelu or gelu")
+        self.config = c = _check_act(_cfg(config, **_TEXT_DEFAULTS))
         self.text_model = _TextTransformer(c)
 
     def _build_pack(self, dev):
-        t = self.text_model
-        return {"tok": _h(t.embeddings.token_embedding.weight, dev), "pos": _h(t.embeddings.position_embedding.weight, dev),
-                "layers": _pack_layers(t.encoder.layers, dev),
-                "final": (_f(t.final_layer_norm.weight, dev), _f(t.final_layer_norm.bias, dev))}
+        return _text_pack(self.text_model, dev)
 
     @torch.no_grad()
     def forward(self, input_ids, output_hidden_states=False, **kwargs):
         P, c = self._packed(), self.config
-        ids = input_ids.to(device=P["tok"].device, dtype=torch.int64).contiguous()
+        last, pos, ids, hidden = _text_forward(P, c, input_ids, output_hidden_states)
         B, n = ids.shape
-        h = torch.empty(B * n, c.hidden_size, dtype=torch.float16, device=ids.device)
-        ops.embed_tokens(ids, P["tok"], P["pos"], h)
-        h, hidden = _run_layers(P["layers"], h, B, n, c.num_attention_heads, _ACT[c.hidden_act], c.layer_norm_eps, causal=True,
-                                keep_hidden=output_hidden_states)
-        last = torch.empty_like(h)
-        ops.layernorm(h, P["final"][0], P["final"][1], last, c.layer_norm_eps)
         last = last.view(B, n, -1).float()
-        # pooled = the features at the end-of-text token (modeling_clip.py: argmax of the ids for the legacy eos id 2)
-        if c.eos_token_id == 2:
-            pos = ids.argmax(dim=-1)
-        else:
-            pos = (ids == c.eos_token_id).int().argmax(dim=-1)
         pooled = last[torch.arange(B, device=ids.device), pos]
         hs = tuple(t.view(B, n, -1).float() for t in hidden) if output_hidden_states else None
         return types.SimpleNamespace(last_hidden_state=last, pooler_output=pooled, hidden_states=hs)
@@ -256,62 +277,204 @@ class _VisionTransformer(nn.Module):
         self.post_layernorm = _Param((c.hidden_size,), kind="norm")
 
 
+def _vision_pack(v, c, dev):
+    k = c.num_channels * c.patch_size ** 2
+    kp = (k + 7) // 8 * 8
+    w = torch.zeros(c.hidden_size, kp, device=dev)
+    w[:, :k] = v.embeddings.patch_embedding.weight.detach().to(dev).float().reshape(c.hidden_size, k)
+    pos = v.embeddings.position_embedding.weight.detach().to(dev).float()
+    return {"patch_w": w.to(torch.float16).contiguous(), "kp": kp, "pos_patches": pos[1:].to(torch.float16).contiguous(),
+            "cls": (v.embeddings.class_embedding.detach().to(dev).float() + pos[0]).to(torch.float16).contiguous(),
+            "pre": (_f(v.pre_layrnorm.weight, dev), _f(v.pre_layrnorm.bias, dev)),
+            "post": (_f(v.post_layernorm.weight, dev), _f(v.post_layernorm.bias, dev)),
+            "layers": _pack_layers(v.encoder.layers, dev)}
+
+
+def _patch_rows(P, c, pixel_values, npos):
+    """pixel_values [B, C, H, W] -> fp16 patch rows [B * patches, kp] (a pure permutation, zero-padded to kp columns)."""
+    dev = P["patch_w"].device
+    x = pixel_values.to(dev)
+    B, Cc, H, W = x.shape
+    p = c.patch_size
+    gh, gw = H // p, W // p
+    assert gh * gw + 1 == npos, "image size does not match the position table"
+    patches = torch.zeros(B * gh * gw, P["kp"], dtype=torch.float16, device=dev)
+    patches[:, : Cc * p * p].copy_(x.reshape(B, Cc, gh, p, gw, p).permute(0, 2, 4, 1, 3, 5).reshape(B * gh * gw, Cc * p * p))
+    return patches
+
+
+def _vision_forward(P, c, patches, keep_hidden=False):
+    """The vision tower from its patch rows [B * patches, kp] fp16 -> (tokens fp16 [B * n, D], post-LayerNorm class token fp16
+    [B, D], hidden states, B, n)."""
+    dev = P["patch_w"].device
+    npatch = P["pos_patches"].shape[0]
+    B = patches.shape[0] // npatch
+    assert tuple(patches.shape) == (B * npatch, P["kp"]) and patches.dtype == torch.float16, "patch rows [B * patches, kp] fp16"
+    D = c.hidden_size
+    emb = torch.empty(B * npatch, D, dtype=torch.float16, device=dev)
+    ops.gemm(patches, P["patch_w"], emb, residual=P["pos_patches"].repeat(B, 1))      # patch conv + position embedding
+    n = npatch + 1
+    tok = torch.empty(B, n, D, dtype=torch.float16, device=dev)
+    tok[:, 0].copy_(P["cls"])
+    tok[:, 1:].copy_(emb.view(B, npatch, D))
+    h = torch.empty(B * n, D, dtype=torch.float16, device=dev)
+    ops.layernorm(tok.view(B * n, D), P["pre"][0], P["pre"][1], h, c.layer_norm_eps)
+    h, hidden = _run_layers(P["layers"], h, B, n, c.num_attention_heads, _ACT[c.hidden_act], c.layer_norm_eps, causal=False,
+                            keep_hidden=keep_hidden)
+    pooled = torch.empty(B, D, dtype=torch.float16, device=dev)
+    ops.layernorm(h.view(B, n, D)[:, 0].contiguous(), P["post"][0], P["post"][1], pooled, c.layer_norm_eps)
+    return h, pooled, hidden, B, n
+
+
+def _project(x16, w):
+    out = torch.empty(x16.shape[0], w.shape[0], dtype=torch.float32, device=x16.device)
+    ops.gemm(x16, w, out)
+    return out
+
+
 class CLIPVisionModelWithProjection(_Packable):
     """``transformers.CLIPVisionModelWithProjection``: ``forward(pixel_values, output_hidden_states=False)`` ->
     namespace(image_embeds, last_hidden_state, hidden_states).  train.py:688-691 consumes ``hidden_states[-2]``."""
 
     def __init__(self, config):
         super().__init__()
-        self.config = c = _cfg(config, hidden_size=1280, intermediate_size=5120, num_hidden_layers=32, num_attention_heads=16,
-                               image_size=224, patch_size=14, num_channels=3, projection_dim=1024, hidden_act="gelu", layer_norm_eps=1e-5)
-        if _ACT.get(c.hidden_act) is None:
-            raise NotImplementedError(f"hidden_act={c.hidden_act!r}: CLIP uses quick_gelu or gelu")
+        self.config = c = _check_act(_cfg(config, **_VISION_DEFAULTS))
         self.vision_model = _VisionTransformer(c)
         self.visual_projection = _Param((c.projection_dim, c.hidden_size), bias=False)
 
     def _build_pack(self, dev):
-        v, c = self.vision_model, self.config
-        k = c.num_channels * c.patch_size ** 2
-        kp = (k + 7) // 8 * 8
-        w = torch.zeros(c.hidden_size, kp, device=dev)
-        w[:, :k] = v.embeddings.patch_embedding.weight.detach().to(dev).float().reshape(c.hidden_size, k)
-        pos = v.embeddings.position_embedding.weight.detach().to(dev).float()
-        return {"patch_w": w.to(torch.float16).contiguous(), "kp": kp, "pos_patches": pos[1:].to(torch.float16).contiguous(),
-                "cls": (v.embeddings.class_embedding.detach().to(dev).float() + pos[0]).to(torch.float16).contiguous(),
-                "pre": (_f(v.pre_layrnorm.weight, dev), _f(v.pre_layrnorm.bias, dev)),
-                "post": (_f(v.post_layernorm.weight, dev), _f(v.post_layernorm.bias, dev)),
-                "layers": _pack_layers(v.encoder.layers, dev), "proj_w": _h(self.visual_projection.weight, dev)}
+        P = _vision_pack(self.vision_model, self.config, dev)
+        P["proj_w"] = _h(self.visual_projection.weight, dev)
+        return P
 
     @torch.no_grad()
     def forward(self, pixel_values, output_hidden_states=False, **kwargs):
         P, c = self._packed(), self.config
-        dev = P["patch_w"].device
-        x = pixel_values.to(dev)
-        B, Cc, H, W = x.shape
-        p = c.patch_size
-        gh, gw = H // p, W // p
-        npatch = gh * gw
-        assert npatch + 1 == self.vision_model.embeddings.position_embedding.weight.shape[0], "image size does not match the position table"
-        # non-overlapping patches -> rows (a pure permutation), zero-padded to a multiple of 8 columns, fp16
-        patches = torch.zeros(B * npatch, P["kp"], dtype=torch.float16, device=dev)
-        patches[:, : Cc * p * p].copy_(x.reshape(B, Cc, gh, p, gw, p).permute(0, 2, 4, 1, 3, 5).reshape(B * npatch, Cc * p * p))
+        patches = _patch_rows(P, c, pixel_values, self.vision_model.embeddings.position_embedding.weight.shape[0])
+        h, pooled, hidden, B, n = _vision_forward(P, c, patches, output_hidden_states)
         D = c.hidden_size
-        emb = torch.empty(B * npatch, D, dtype=torch.float16, device=dev)
-        ops.gemm(patches, P["patch_w"], emb, residual=P["pos_patches"].repeat(B, 1))      # patch conv + position embedding
-        n = npatch + 1
-        tok = torch.empty(B, n, D, dtype=torch.float16, device=dev)
-        tok[:, 0].copy_(P["cls"])
-        tok[:, 1:].copy_(emb.view(B, npatch, D))
-        h = torch.empty(B * n, D, dtype=torch.float16, device=dev)
-        ops.layernorm(tok.view(B * n, D), P["pre"][0], P["pre"][1], h, c.layer_norm_eps)
-        h, hidden = _run_layers(P["layers"], h, B, n, c.num_attention_heads, _ACT[c.hidden_act], c.layer_norm_eps, causal=False,
-                                keep_hidden=output_hidden_states)
-        pooled = torch.empty(B, D, dtype=torch.float16, device=dev)
-        ops.layernorm(h.view(B, n, D)[:, 0].contiguous(), P["post"][0], P["post"][1], pooled, c.layer_norm_eps)
-        embeds = torch.empty(B, P["proj_w"].shape[0], dtype=torch.float32, device=dev)
-        ops.gemm(pooled, P["proj_w"], embeds)
+        embeds = _project(pooled, P["proj_w"])
         hs = tuple(t.view(B, n, D).float() for t in hidden) if output_hidden_states else None
         return types.SimpleNamespace(image_embeds=embeds, last_hidden_state=h.view(B, n, D).float(), hidden_states=hs)
+
+
+class CLIPModel(_Packable):
+    """``transformers.CLIPModel`` (modeling_clip.py) under its state-dict keys (``text_model.*``, ``vision_model.*``,
+    ``visual_projection.weight``, ``text_projection.weight``, ``logit_scale``).  ``config``: dict or ``CLIPConfig`` with
+    ``text_config`` / ``vision_config`` (dicts or configs) and ``projection_dim``.
+    ``get_text_features(input_ids)`` / ``get_image_features(pixel_values)`` -> the projected, un-normalised fp32 embeddings;
+    ``get_image_features(patch_rows=...)`` takes the fp16 patch rows of ``ops.clip_preprocess`` instead of pixels."""
+
+    def __init__(self, config):
+        super().__init__()
+        c = _cfg(config, text_config={}, vision_config={}, projection_dim=512, logit_scale_init_value=2.6592)
+        tc, vc = c.text_config, c.vision_config
+        self.text_config = _check_act(_cfg(tc, **_TEXT_DEFAULTS))
+        self.vision_config = _check_act(_cfg(vc, **_VISION_DEFAULTS))
+        self.projection_dim = c.projection_dim
+        self.text_model = _TextTransformer(self.text_config)
+        self.vision_model = _VisionTransformer(self.vision_config)
+        self.visual_projection = _Param((c.projection_dim, self.vision_config.hidden_size), bias=False)
+        self.text_projection = _Param((c.projection_dim, self.text_config.hidden_size), bias=False)
+        self.logit_scale = nn.Parameter(torch.tensor(float(c.logit_scale_init_value)))
+
+    def _build_pack(self, dev):
+        return {"text": _text_pack(self.text_model, dev), "vision": _vision_pack(self.vision_model, self.vision_config, dev),
+                "vproj": _h(self.visual_projection.weight, dev), "tproj": _h(self.text_projection.weight, dev),
+                "logit_scale": float(self.logit_scale.detach().float().cpu())}
+
+    @property
+    def patch_size(self):
+        return self.vision_config.patch_size
+
+    @torch.no_grad()
+    def get_text_features(self, input_ids):
+        P = self._packed()
+        last, pos, ids, _ = _text_forward(P["text"], self.text_config, input_ids)
+        B, n = ids.shape
+        pooled = last.view(B, n, -1)[torch.arange(B, device=ids.device), pos].contiguous()
+        return _project(pooled, P["tproj"])
+
+    @torch.no_grad()
+    def get_image_features(self, pixel_values=None, patch_rows=None):
+        P = self._packed()
+        if patch_rows is None:
+            patch_rows = _patch_rows(P["vision"], self.vision_config, pixel_values,
+                                     self.vision_model.embeddings.position_embedding.weight.shape[0])
+        _, pooled, _, _, _ = _vision_forward(P["vision"], self.vision_config, patch_rows)
+        return _project(pooled, P["vproj"])
+
+    def logit_scale_value(self):
+        return self._packed()["logit_scale"]
+
+
+# OpenAI ``clip.load`` state dict <-> ``transformers.CLIPModel`` keys.  in_proj_* of every residual block is split into
+# q / k / v; ``visual.proj`` and ``text_projection`` are stored transposed ([width, embed]).
+_OA_TOP = (("visual.conv1.weight", "vision_model.embeddings.patch_embedding.weight"),
+           ("visual.class_embedding", "vision_model.embeddings.class_embedding"),
+           ("visual.positional_embedding", "vision_model.embeddings.position_embedding.weight"),
+           ("visual.ln_pre.", "vision_model.pre_layrnorm."), ("visual.ln_post.", "vision_model.post_layernorm."),
+           ("token_embedding.weight", "text_model.embeddings.token_embedding.weight"),
+           ("positional_embedding", "text_model.embeddings.position_embedding.weight"),
+           ("ln_final.", "text_model.final_layer_norm."), ("logit_scale", "logit_scale"))
+_OA_BLOCK = (("ln_1.", "layer_norm1."), ("ln_2.", "layer_norm2."), ("attn.out_proj.", "self_attn.out_proj."),
+             ("mlp.c_fc.", "mlp.fc1."), ("mlp.c_proj.", "mlp.fc2."))
+_OA_TOWER = (("visual.transformer.resblocks.", "vision_model.encoder.layers."), ("transformer.resblocks.", "text_model.encoder.layers."))
+_OA_META = ("input_resolution", "context_length", "vocab_size")      # integer attributes some checkpoints carry
+
+
+def openai_clip_to_transformers(sd):
+    """State dict of OpenAI's ``clip`` model (``clip.load(...)[0].state_dict()``) -> ``transformers.CLIPModel`` keys."""
+    out = {}
+    for k, v in sd.items():
+        if k in _OA_META:
+            continue
+        if k == "visual.proj":
+            out["visual_projection.weight"] = v.t().contiguous()
+            continue
+        if k == "text_projection":
+            out["text_projection.weight"] = v.t().contiguous()
+            continue
+        for a, b in _OA_TOWER:
+            m = re.fullmatch(re.escape(a) + r"(\d+)\.(.*)", k)
+            if m:
+                pre, rest = f"{b}{m.group(1)}.", m.group(2)
+                if rest.startswith("attn.in_proj_"):
+                    leaf = "weight" if rest.endswith("weight") else "bias"
+                    for n, t in zip(("q_proj", "k_proj", "v_proj"), v.chunk(3, 0)):
+                        out[f"{pre}self_attn.{n}.{leaf}"] = t.contiguous()
+                else:
+                    out[pre + _rename(rest, _OA_BLOCK, "CLIP")] = v
+                break
+        else:
+            out[_rename(k, _OA_TOP, "CLIP")] = v
+    return out
+
+
+def transformers_to_openai_clip(sd):
+    """Inverse of ``openai_clip_to_transformers``."""
+    out = {}
+    for k, v in sd.items():
+        if k == "visual_projection.weight":
+            out["visual.proj"] = v.t().contiguous()
+            continue
+        if k == "text_projection.weight":
+            out["text_projection"] = v.t().contiguous()
+            continue
+        for a, b in _OA_TOWER:
+            m = re.fullmatch(re.escape(b) + r"(\d+)\.(.*)", k)
+            if m:
+                pre, rest = f"{a}{m.group(1)}.", m.group(2)
+                if rest.startswith("self_attn.q_proj."):
+                    leaf = rest.rsplit(".", 1)[1]
+                    base = f"{b}{m.group(1)}.self_attn."
+                    out[f"{pre}attn.in_proj_{leaf}"] = torch.cat([sd[f"{base}{n}.{leaf}"] for n in ("q_proj", "k_proj", "v_proj")], 0)
+                elif not rest.startswith(("self_attn.k_proj.", "self_attn.v_proj.")):
+                    out[pre + _rename(rest, tuple((y, x) for x, y in _OA_BLOCK), "CLIP")] = v
+                break
+        else:
+            out[_rename(k, tuple((y, x) for x, y in _OA_TOP), "CLIP")] = v
+    return out
 
 
 # ---- DINOv2 ViT-g/14: AnyDoor's reference-image encoder -------------------------------------------------------------------------
@@ -347,11 +510,11 @@ _HF_BLOCK = (("norm1.", "norm1."), ("attention.output.dense.", "attn.proj."), ("
 _QKV = ("query", "key", "value")
 
 
-def _rename(k, table):
+def _rename(k, table, what="DINOv2"):
     for a, b in table:
         if k.startswith(a):
             return b + k[len(a):]
-    raise KeyError(f"no DINOv2 key mapping for {k!r}")
+    raise KeyError(f"no {what} key mapping for {k!r}")
 
 
 def dinov2_from_transformers(sd):

@@ -723,6 +723,102 @@ def anydoor_crop_back(src, tar_images, geom, out):
                "anydoor_crop_back")
     _count()
 
+
+# ---- post-filter scores (filter_tool/utils.py) ---------------------------------------------------------------------------
+CLIP_CROP = {"floor": 0, "round": 1}      # transformers' center_crop / torchvision's CenterCrop
+
+
+def clip_preprocess_plan(sizes, crop, patch, channels=3):
+    """Host-side plan of ``clip_preprocess``: sizes = [(H, W), ...] -> (int32 table as a CPU tensor, rows per CTA, shared bytes).
+    Raises ValueError on an unknown crop mode, a patch size other than 14 / 32, a non-RGB input or an empty image."""
+    if crop not in CLIP_CROP:
+        raise ValueError(f"crop={crop!r}: 'floor' (transformers) or 'round' (torchvision)")
+    B = len(sizes)
+    hw = (C.c_int * max(2 * B, 1))(*[int(v) for s in sizes for v in s])
+    n, R, sm = C.c_longlong(0), C.c_int(0), C.c_int(0)
+    lib = _lib.load()
+    args = (hw, B, int(channels), CLIP_CROP[crop], int(patch))
+    _lib.check(lib.anysd_clip_preprocess_plan(*args, None, C.byref(n), C.byref(R), C.byref(sm)), "clip_preprocess_plan")
+    table = torch.empty(n.value, dtype=torch.int32, pin_memory=torch.cuda.is_available())
+    _lib.check(lib.anysd_clip_preprocess_plan(*args, C.cast(table.data_ptr(), C.POINTER(C.c_int)), C.byref(n), C.byref(R),
+                                              C.byref(sm)), "clip_preprocess_plan")
+    return table, R.value, sm.value
+
+
+def _ptr_table(ts, dev):
+    return torch.tensor([t.data_ptr() for t in ts], dtype=torch.int64).pin_memory().to(dev, non_blocking=True)
+
+
+def clip_preprocess(images, lut, patch, crop, rows=None, crop_u8=None):
+    """The CLIP preprocessors from image bytes, one launch for B images of any sizes: uint8 HWC RGB CUDA tensors -> the fp16
+    patch rows [B * (224 / patch)^2, kp] of the vision tower (``rows``, allocated when None) of the 224 x 224 crop of Pillow's
+    bicubic resize to short side 224; ``lut`` fp16 [3, 256] is the processor's normalised value of each byte
+    (``postfilter.pixel_lut``).  ``crop_u8`` (optional, uint8 [B, 224, 224, 3]) receives the crop's bytes."""
+    if not images:
+        raise ValueError("clip_preprocess: no images")
+    _cuda(*images, lut, rows, crop_u8)
+    for im in images:
+        if im.dtype != torch.uint8 or im.dim() != 3 or not im.is_contiguous():
+            raise ValueError("clip_preprocess: images are contiguous uint8 [H, W, C] tensors")
+    channels = images[0].shape[2] if all(im.shape[2] == images[0].shape[2] for im in images) else -1
+    table, R, sm = clip_preprocess_plan([tuple(im.shape[:2]) for im in images], crop, patch, channels)
+    dev = images[0].device
+    B, g = len(images), 224 // patch
+    kp = (3 * patch * patch + 7) // 8 * 8
+    if rows is None:
+        rows = torch.empty(B * g * g, kp, dtype=torch.float16, device=dev)
+    assert rows.dtype == torch.float16 and rows.is_contiguous() and tuple(rows.shape) == (B * g * g, kp)
+    assert lut.dtype == torch.float16 and lut.is_contiguous() and lut.numel() == 768
+    if crop_u8 is not None:
+        assert crop_u8.dtype == torch.uint8 and crop_u8.is_contiguous() and tuple(crop_u8.shape) == (B, 224, 224, 3)
+    table = table.to(dev, non_blocking=True)
+    ptrs = _ptr_table(images, dev)
+    _lib.check(_lib.load().anysd_clip_preprocess_u8(_ptr(ptrs), _ptr(table), B, int(patch), R, sm, _ptr(lut), _ptr(rows),
+                                                    _ptr(crop_u8), _stream()), "clip_preprocess")
+    _count()
+    return rows
+
+
+def l1_wrapped_sum(originals, edited):
+    """Per pair, the exact sum of (a - b) mod 256 over the bytes (numpy's uint8 ``np.sum(np.abs(a - b))``) -> int64 [B] CUDA
+    tensor.  Shapes must match pair by pair (ValueError otherwise, as numpy raises)."""
+    if len(originals) != len(edited) or not originals:
+        raise ValueError("l1_wrapped_sum: need the same positive number of originals and edited images")
+    _cuda(*originals, *edited)
+    for a, b in zip(originals, edited):
+        if a.shape != b.shape:
+            raise ValueError(f"operands could not be broadcast together with shapes {tuple(a.shape)} {tuple(b.shape)}")
+        if a.dtype != torch.uint8 or b.dtype != torch.uint8 or not (a.is_contiguous() and b.is_contiguous()):
+            raise ValueError("l1_wrapped_sum: images are contiguous uint8 tensors")
+    dev = originals[0].device
+    n = [a.numel() for a in originals]
+    if min(n) < 1:
+        raise ValueError("l1_wrapped_sum: empty image")
+    nbytes = torch.tensor(n, dtype=torch.int64).pin_memory().to(dev, non_blocking=True)
+    out = torch.empty(len(n), dtype=torch.int64, device=dev)
+    pa, pb = _ptr_table(originals, dev), _ptr_table(edited, dev)      # held until the launch: the allocator would reuse a freed table
+    _lib.check(_lib.load().anysd_l1_wrapped_u8(_ptr(pa), _ptr(pb), _ptr(nbytes), len(n), max(n), _ptr(out), _stream()), "l1_wrapped_sum")
+    _count()
+    return out
+
+
+def postfilter_scores(out, img_h=None, txt_h=None, logit_scale=0.0, img_a=None, img_b=None, txt_a=None, txt_b=None):
+    """out fp32 [B, 2] <- (exp(logit_scale) cos(img_h, txt_h) / 100, cos(img_b - img_a, txt_b - txt_a), 0 for a zero
+    difference); features fp32 [B, E]; a group left None leaves its column alone."""
+    ts = (img_h, txt_h, img_a, img_b, txt_a, txt_b)
+    _cuda(out, *ts)
+    B = out.shape[0]
+    assert out.dtype == torch.float32 and out.is_contiguous() and tuple(out.shape) == (B, 2)
+    for t in ts:
+        assert t is None or (t.dtype == torch.float32 and t.is_contiguous() and t.dim() == 2 and t.shape[0] == B)
+    E1 = img_h.shape[1] if img_h is not None else 0
+    E2 = img_a.shape[1] if img_a is not None else 0
+    assert txt_h is None or txt_h.shape[1] == E1
+    assert all(t is None or t.shape[1] == E2 for t in (img_b, txt_a, txt_b))
+    _lib.check(_lib.load().anysd_postfilter_scores_f32(_ptr(img_h), _ptr(txt_h), E1, float(logit_scale), _ptr(img_a), _ptr(img_b),
+                                                       _ptr(txt_a), _ptr(txt_b), E2, B, _ptr(out), _stream()), "postfilter_scores")
+    _count()
+
 # ---- training step (SURVEY.md a24): thin wrappers, same conventions as above -------------------------------------
 def q_sample(x0, noise, t, sqrt_acp, sqrt_1m_acp, out):
     _cuda(x0, noise, t, out)

@@ -371,6 +371,34 @@ int anysd_anydoor_sobel(const void* ref_u8, const void* mask_u8, int B, void* im
 int anysd_anydoor_crop_back(const void* src, int decoded, const void* tar_img, int B, int H, int W, const void* geom, void* out,
                             anysd_stream_t stream);
 
+/* ---- AnyEdit's post-filter scores (AnyEdit_Collection/filter_tool/utils.py get_clip_score, get_directional_clip,
+ * get_L1_distance; DESIGN.md §10.10).
+ * anysd_clip_preprocess_plan (host only, no CUDA call): images of sizes hw [B, 2] (host int32 H, W), channels (must be 3) ->
+ * the int32 table the kernel reads: per image a row of CLIP_PRE_G = (H, W, x entries offset, x stride, y entries offset,
+ * y stride, 0, 0), then for each of the 224 crop columns / rows (min, count, 22-bit coefficients) of Pillow's bicubic resize
+ * to short side 224 (long side int(224 * long / short)), centre-cropped with CLIP_CROP_FLOOR (transformers: (h - 224) // 2) or
+ * CLIP_CROP_ROUND (torchvision: round((h - 224) / 2), half to even).  table = NULL sizes it (*table_ints); *rows_per_cta and
+ * *smem_bytes are the launch plan.  patch: 14 or 32.
+ * anysd_clip_preprocess_u8: images = device array of B pointers to uint8 HWC RGB images, table = the plan on the device,
+ * lut = fp16 [3, 256], the preprocessor's normalised value of each byte -> rows fp16 [B * (224 / patch)^2, kp] (kp = 3 patch^2
+ * rounded up to 8, padding zeroed), the patch rows of the vision tower's patch contraction (columns channel, y, x); crop_u8
+ * (optional) uint8 [B, 224, 224, 3] the resized crop, equal to PIL.Image.resize(BICUBIC) on every byte.
+ * anysd_l1_wrapped_u8: a, b = device arrays of B pointers to uint8 images, nbytes = device int64 [B] -> out uint64 [B] =
+ * sum of (a - b) mod 256 over each pair's bytes (numpy's uint8 np.abs(a - b)); max_bytes bounds every nbytes.
+ * anysd_postfilter_scores_f32 (one launch, B pairs): out fp32 [B, 2] = (exp(logit_scale) cos(img_h, txt_h) / 100,
+ * cos(img_b - img_a, txt_b - txt_a), 0 when a difference is exactly zero); either group of features may be NULL (its
+ * column is not written).  Features fp32 [B, E1] / [B, E2]. */
+#define CLIP_PRE_G 8
+#define CLIP_CROP_FLOOR 0
+#define CLIP_CROP_ROUND 1
+int anysd_clip_preprocess_plan(const int* hw, int B, int channels, int crop_mode, int patch, int* table, long long* table_ints,
+                               int* rows_per_cta, int* smem_bytes);
+int anysd_clip_preprocess_u8(const void* images, const void* table, int B, int patch, int rows_per_cta, int smem_bytes, const void* lut,
+                             void* rows, void* crop_u8, anysd_stream_t stream);
+int anysd_l1_wrapped_u8(const void* a, const void* b, const void* nbytes, int B, long long max_bytes, void* out, anysd_stream_t stream);
+int anysd_postfilter_scores_f32(const float* img_h, const float* txt_h, int E1, float logit_scale, const float* img_a, const float* img_b,
+                                const float* txt_a, const float* txt_b, int E2, int B, float* out, anysd_stream_t stream);
+
 /* ==== training step (SURVEY.md a24; train.py:629-710) =====================================================
  * The reference back-propagates mse_loss(MoE(...), noise) through the frozen UNet with torch autograd
  * (train.py:694-703); trainables are the adapter experts, the router and the task-embedding table
