@@ -130,6 +130,12 @@ SIGNATURES = {
     "anysd_clip_preprocess_u8": (_I, [_VP, _VP, _I, _I, _I, _I, _VP, _VP, _VP, _VP]),
     "anysd_l1_wrapped_u8": (_I, [_VP, _VP, _VP, _I, _LL, _VP, _VP]),
     "anysd_postfilter_scores_f32": (_I, [_VP, _VP, _I, _F, _VP, _VP, _VP, _VP, _I, _I, _VP, _VP]),
+    # ---- inpainting edits ----
+    "anysd_pil_resize_plan": (_I, [C.POINTER(_I), C.POINTER(_I), _I, _I, C.POINTER(_I), C.POINTER(_LL), C.POINTER(_I), C.POINTER(_I),
+                                   C.POINTER(_I)]),
+    "anysd_pil_resize_u8": (_I, [_VP, _VP, _VP, _I, _I, _I, _I, _I, _VP]),
+    "anysd_inpaint_prepare": (_I, [_VP, _VP, _I, _I, _I, _I, _VP, _VP, _VP, _VP]),
+    "anysd_background_mask_u8": (_I, [_VP, _VP, _VP, _I, _I, _I, _VP, _VP]),
     # ---- training step ----
     "anysd_q_sample_f32": (_I, [_VP, _VP, _VP, _VP, _VP, _VP, _I, _LL, _VP]),
     "anysd_mse_workspace_bytes": (_SZ, []),

@@ -323,17 +323,32 @@ class AutoencoderKL(nn.Module):
     @torch.no_grad()
     def encode(self, x):
         """autoencoder.py:82-86: Encoder -> quant_conv -> DiagonalGaussianDistribution(moments)."""
-        P = self._prepare()
-        E = P["enc"]
-        dev = x.device
-        if dev.type != "cuda":
+        if x.device.type != "cuda":
             raise RuntimeError("anyedit_b200.AutoencoderKL: input must be a CUDA tensor (no CPU fallback)")
         N, Cin, H, W = x.shape
         assert Cin == self.encoder.in_channels
+        xin = torch.zeros(N, H, W, self.input_row_channels, dtype=torch.float16, device=x.device)
+        ops.nchw_to_nhwc(x.float().contiguous(), xin, 0)
+        return self.encode_rows(xin)
+
+    @property
+    def input_row_channels(self):
+        """Channels per pixel of the encoder's fp16 NHWC input rows: the image's, zero-padded to a multiple of 64."""
+        return (self.encoder.in_channels + 63) // 64 * 64
+
+    @torch.no_grad()
+    def encode_rows(self, xin):
+        """``encode`` of the encoder's own input rows: fp16 NHWC [N, H, W, ``input_row_channels``], zeros after the image
+        channels (what ``ops.inpaint_prepare`` writes)."""
+        P = self._prepare()
+        E = P["enc"]
+        dev = xin.device
+        N, H, W, cp = xin.shape
+        if dev.type != "cuda" or xin.dtype != torch.float16 or cp != E["cin_pad"] or not xin.is_contiguous():
+            raise ValueError(f"encode_rows: contiguous fp16 CUDA rows [N, H, W, {E['cin_pad']}]")
+        Cin = self.encoder.in_channels
         f16 = dict(dtype=torch.float16, device=dev)
         ws = ops.groupnorm_workspace(N, 32, 0, dev)
-        xin = torch.zeros(N, H, W, E["cin_pad"], **f16)
-        ops.nchw_to_nhwc(x.float().contiguous(), xin, 0)
         ch = self.encoder.ch
         h = torch.empty(N, H, W, ch, **f16)
         ops.conv3x3(xin, E["conv_in"]["w"], h.view(-1, ch), bias=E["conv_in"]["b"], logical_cin=Cin)

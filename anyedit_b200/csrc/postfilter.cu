@@ -2,8 +2,7 @@
 // DESIGN.md §10.10).
 //   anysd_clip_preprocess_plan  host only: per image, the resized size (short side 224, long side int(224 * long / short)), the
 //                               224 x 224 crop offsets (transformers' floor or torchvision's round-half-even) and Pillow's
-//                               bicubic coefficients for the crop's columns and rows, in Pillow's double operation order
-//                               and its 22-bit fixed point
+//                               bicubic coefficients for the crop's columns and rows (pil_resample.cuh)
 //   clip_preprocess_kernel      one CTA per image x band of output rows: the horizontal pass of the band's source rows as
 //                               clipped uint8 in shared memory, the vertical pass, a per-channel fp16 table -> the patch rows
 //                               of the vision tower's patch contraction (and optionally the crop's bytes)
@@ -16,61 +15,13 @@
 #include <vector>
 
 #include "common.cuh"
+#include "pil_resample.cuh"
 
 namespace anysd {
 
 namespace {
 
-constexpr int CROP = 224, PREC = 22, PRE_THREADS = 256, SMEM_MAX = 200 * 1024;
-
-// Pillow's bicubic filter, a = -0.5
-double bicubic(double x) {
-    const double a = -0.5;
-    if (x < 0.0) x = -x;
-    if (x < 1.0) return ((a + 2.0) * x - (a + 3.0)) * x * x + 1.0;
-    if (x < 2.0) return (((x - 5.0) * x + 8.0) * x - 4.0) * a;
-    return 0.0;
-}
-
-// One axis in -> out: for output positions [first, first + n) the entries (min, count, c_0 .. c_{k-1}) of stride 2 + k.  A pass
-// whose size does not change is the identity (Pillow skips it; one coefficient of 1 << 22 reproduces the skip exactly).
-int axis_coeffs(int in, int out, int first, int n, std::vector<int>* dst) {
-    if (in == out) {
-        if (dst)
-            for (int i = 0; i < n; ++i) dst->insert(dst->end(), {first + i, 1, 1 << PREC});
-        return 1;
-    }
-    const double scale = (double)in / (double)out;
-    const double filterscale = scale < 1.0 ? 1.0 : scale;
-    const double support = 2.0 * filterscale;
-    const int ksize = (int)ceil(support) * 2 + 1;
-    if (!dst) return ksize;
-    std::vector<double> k(ksize);
-    for (int i = 0; i < n; ++i) {
-        const int xx = first + i;
-        const double center = (xx + 0.5) * scale;
-        const double ss = 1.0 / filterscale;
-        int xmin = (int)(center - support + 0.5);
-        if (xmin < 0) xmin = 0;
-        int xmax = (int)(center + support + 0.5);
-        if (xmax > in) xmax = in;
-        xmax -= xmin;
-        double ww = 0.0;
-        for (int x = 0; x < xmax; ++x) {
-            const double w = bicubic((x + xmin - center + 0.5) * ss);
-            k[x] = w;
-            ww += w;
-        }
-        dst->push_back(xmin);
-        dst->push_back(xmax);
-        for (int x = 0; x < ksize; ++x) {
-            double w = x < xmax ? k[x] : 0.0;
-            if (x < xmax && ww != 0.0) w /= ww;
-            dst->push_back(w < 0 ? (int)(-0.5 + w * (1 << PREC)) : (int)(0.5 + w * (1 << PREC)));
-        }
-    }
-    return ksize;
-}
+constexpr int CROP = 224, PREC = PIL_PREC, PRE_THREADS = 256, SMEM_MAX = 200 * 1024;
 
 __device__ __forceinline__ int clip8(int s) {
     s >>= PREC;
@@ -255,13 +206,13 @@ int anysd_clip_preprocess_plan(const int* hw, int B, int channels, int crop_mode
         int* g = &t[(size_t)b * CLIP_PRE_G];
         g[0] = H, g[1] = W;
         g[2] = (int)t.size();
-        const int kx = axis_coeffs(W, rw, left, CROP, nullptr);
-        axis_coeffs(W, rw, left, CROP, &t);
+        const int kx = pil_axis_coeffs(PIL_BICUBIC, W, rw, left, CROP, nullptr);
+        pil_axis_coeffs(PIL_BICUBIC, W, rw, left, CROP, &t);
         g = &t[(size_t)b * CLIP_PRE_G];
         g[3] = 2 + kx;
         g[4] = (int)t.size();
-        const int ky = axis_coeffs(H, rh, top, CROP, nullptr);
-        axis_coeffs(H, rh, top, CROP, &t);
+        const int ky = pil_axis_coeffs(PIL_BICUBIC, H, rh, top, CROP, nullptr);
+        pil_axis_coeffs(PIL_BICUBIC, H, rh, top, CROP, &t);
         g = &t[(size_t)b * CLIP_PRE_G];
         g[5] = 2 + ky;
         ANYSD_REQUIRE(t.size() < (1u << 31), ANYSD_EINVAL, "clip_preprocess_plan: table too large");

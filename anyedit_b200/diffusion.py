@@ -184,3 +184,37 @@ class LatentDenoiser(nn.Module):
         if isinstance(x_recon, tuple) and not return_ids:
             return x_recon[0]
         return x_recon
+
+
+class LatentInpaintDenoiser(LatentDenoiser):
+    """ldm's ``LatentInpaintDiffusion`` (ddpm.py:1646-1690) on the sampler side: a ``hybrid`` denoiser whose UNet input is
+    ``cat([x, mask, masked_image latents])`` in the order of ``concat_keys`` (the ``sd-v1-5-inpainting`` / ``sd-inpaint``
+    layout: 9 UNet input channels).  The state dict is ldm's (``model.diffusion_model.*``, ``first_stage_model.*``), so the
+    released checkpoint's ``state_dict`` loads with ``load_state_dict(..., strict=False)`` (the text encoder's keys are left
+    over).  ``anyedit_b200.inpaint`` builds the concatenated channels."""
+
+    # ldm yaml params (ddpm.py LatentDiffusion / LatentFinetuneDiffusion) that only concern training, logging or the stages
+    # this class takes as modules: accepted and not used.  first_stage_config / cond_stage_config are not instantiated: pass
+    # the built ``first_stage_model``; the text encoder stays outside the sampler path.
+    _LDM_UNUSED = ("first_stage_config", "cond_stage_config", "first_stage_key", "cond_stage_key", "cond_stage_trainable",
+                   "cond_stage_forward", "image_size", "channels", "monitor", "use_ema", "scale_by_std", "finetune_keys",
+                   "keep_finetune_dims", "c_concat_log_start", "c_concat_log_end", "log_every_t", "scheduler_config",
+                   "use_positional_encodings", "learn_logvar", "logvar_init", "loss_type", "load_only_unet", "ckpt_path",
+                   "ignore_keys", "clip_denoised", "v_posterior", "l_simple_weight", "original_elbo_weight", "num_timesteps_cond")
+
+    def __init__(self, unet_config, concat_keys=("mask", "masked_image"), masked_image_key="masked_image", conditioning_key="hybrid",
+                 **kwargs):
+        unknown = sorted(set(kwargs) - set(self._LDM_UNUSED) - {
+            "timesteps", "beta_schedule", "linear_start", "linear_end", "cosine_s", "parameterization", "given_betas",
+            "first_stage_model", "scale_factor"})
+        if unknown:
+            raise TypeError(f"LatentInpaintDiffusion: unexpected params {unknown}")
+        kwargs = {k: v for k, v in kwargs.items() if k not in self._LDM_UNUSED}
+        concat_keys = tuple(concat_keys)
+        if masked_image_key not in concat_keys:
+            raise ValueError(f"masked_image_key {masked_image_key!r} is not one of concat_keys {concat_keys}")
+        if concat_keys != ("mask", "masked_image") or conditioning_key != "hybrid":
+            raise NotImplementedError("LatentInpaintDiffusion: the mask + masked-image concatenation with hybrid conditioning "
+                                      "(the SD inpainting checkpoints) is implemented")
+        super().__init__(unet_config, conditioning_key=conditioning_key, **kwargs)
+        self.concat_keys, self.masked_image_key = concat_keys, masked_image_key

@@ -819,6 +819,88 @@ def postfilter_scores(out, img_h=None, txt_h=None, logit_scale=0.0, img_a=None, 
                                                        _ptr(txt_a), _ptr(txt_b), E2, B, _ptr(out), _stream()), "postfilter_scores")
     _count()
 
+# ---- inpainting edits (local_pipeline_tool.py, StableDiffusionInpaintPipeline) ---------------------------------------------
+PIL_FILTER = {"nearest": 0, "lanczos": 1, "bicubic": 3, "mode1": 16}     # PIL_RESAMPLE_* in include/anysd_b200.h
+
+
+def pil_resize_plan(sizes, filters, channels):
+    """Host-side plan of ``pil_resize``: sizes = [(H, W, OH, OW), ...], filters = names of ``PIL_FILTER`` per image -> (int32
+    table as a CPU tensor, rows per CTA, shared bytes, bands).  Raises ValueError on a bad size, filter or channel count."""
+    B = len(sizes)
+    if any(f not in PIL_FILTER for f in filters) or len(filters) != B:
+        raise ValueError(f"pil_resize: one filter per image from {sorted(PIL_FILTER)}")
+    sz = (C.c_int * max(4 * B, 1))(*[int(v) for s in sizes for v in s])
+    fl = (C.c_int * max(B, 1))(*[PIL_FILTER[f] for f in filters])
+    n, R, sm, nb = C.c_longlong(0), C.c_int(0), C.c_int(0), C.c_int(0)
+    lib = _lib.load()
+    args = (sz, fl, B, int(channels))
+    _lib.check(lib.anysd_pil_resize_plan(*args, None, C.byref(n), C.byref(R), C.byref(sm), C.byref(nb)), "pil_resize_plan")
+    table = torch.empty(n.value, dtype=torch.int32, pin_memory=torch.cuda.is_available())
+    _lib.check(lib.anysd_pil_resize_plan(*args, C.cast(table.data_ptr(), C.POINTER(C.c_int)), C.byref(n), C.byref(R), C.byref(sm),
+                                         C.byref(nb)), "pil_resize_plan")
+    return table, R.value, sm.value, nb.value
+
+
+def pil_resize(images, outs, filters):
+    """Pillow's ``Image.resize`` of B uint8 HWC images of any sizes in one launch, equal to Pillow on every byte: ``images[i]``
+    [H, W, C] -> ``outs[i]`` [OH, OW, C] (preallocated), C = 3 (RGB) or 1 (L / mode "1") for all; ``filters[i]`` a name of
+    ``PIL_FILTER`` ("mode1": a mode "1" image as 0/1 bytes -- a bool tensor viewed as uint8; other values are outside the
+    contract -- NEAREST and convert("L"), so 0 / 255).  The kernel stages a band of source rows x output width in shared memory
+    (at most 200 KB): an RGB LANCZOS upscale to more than about 9 500 columns raises ValueError."""
+    if not images or len(outs) != len(images):
+        raise ValueError("pil_resize: as many outputs as images, at least one")
+    _cuda(*images, *outs)
+    for a, o in zip(images, outs):
+        if a.dtype != torch.uint8 or o.dtype != torch.uint8 or a.dim() != 3 or o.dim() != 3 or not (a.is_contiguous() and o.is_contiguous()):
+            raise ValueError("pil_resize: contiguous uint8 [H, W, C] tensors")
+        if a.shape[2] != images[0].shape[2] or o.shape[2] != a.shape[2]:
+            raise ValueError("pil_resize: one channel count for the whole batch")
+    Cc = images[0].shape[2]
+    table, R, sm, nb = pil_resize_plan([(*a.shape[:2], *o.shape[:2]) for a, o in zip(images, outs)], filters, Cc)
+    dev = images[0].device
+    table = table.to(dev, non_blocking=True)
+    src, dst = _ptr_table(images, dev), _ptr_table(outs, dev)
+    _lib.check(_lib.load().anysd_pil_resize_u8(_ptr(src), _ptr(dst), _ptr(table), len(images), Cc, R, sm, nb, _stream()), "pil_resize")
+    _count()
+
+
+def inpaint_prepare(img, mask, masked, mask_latent, counts):
+    """The inpaint pipeline's conditioning of B requests in one launch: uint8 img [B, H, W, 3], mask [B, H, W] (the processors'
+    resized bytes) -> masked fp16 [B, H, W, ldc] (the encoder's input rows: fp16 of (x / 255 * 2 - 1) * (mask < 128), zeros
+    after channel 3), mask_latent fp32 [B, 1, H / 8, W / 8] (mask[8i, 8j] >= 128) and counts int32 [B] (bytes >= 128)."""
+    _cuda(img, mask, masked, mask_latent, counts)
+    B, H, W, _ = img.shape
+    assert img.dtype == mask.dtype == torch.uint8 and tuple(img.shape) == (B, H, W, 3) and tuple(mask.shape) == (B, H, W)
+    assert masked.dtype == torch.float16 and masked.dim() == 4 and tuple(masked.shape[:3]) == (B, H, W)
+    assert mask_latent.dtype == torch.float32 and tuple(mask_latent.shape) == (B, 1, H // 8, W // 8)
+    assert counts.dtype == torch.int32 and tuple(counts.shape) == (B,)
+    assert all(t.is_contiguous() for t in (img, mask, masked, mask_latent, counts))
+    _lib.check(_lib.load().anysd_inpaint_prepare(_ptr(img), _ptr(mask), B, H, W, masked.shape[3], _ptr(masked), _ptr(mask_latent),
+                                                 _ptr(counts), _stream()), "inpaint_prepare")
+    _count()
+
+
+def background_mask(images, outs, counts):
+    """background_change's mask of B BGR uint8 images [H, W, 3] of any sizes in one launch: ``outs[i]`` uint8 [H, W] =
+    (cvtColor(GaussianBlur(img, (5, 5), 0), BGR2GRAY) == 0), OpenCV's bytes; counts int32 [B] = the ones of each."""
+    if not images or len(outs) != len(images):
+        raise ValueError("background_mask: as many outputs as images, at least one")
+    _cuda(*images, *outs, counts)
+    for a, o in zip(images, outs):
+        if a.dtype != torch.uint8 or a.dim() != 3 or a.shape[2] != 3 or not a.is_contiguous():
+            raise ValueError("background_mask: images are contiguous uint8 [H, W, 3] (BGR) tensors")
+        if o.dtype != torch.uint8 or tuple(o.shape) != tuple(a.shape[:2]) or not o.is_contiguous():
+            raise ValueError("background_mask: outputs are contiguous uint8 [H, W] tensors of their image's size")
+    B = len(images)
+    assert counts.dtype == torch.int32 and tuple(counts.shape) == (B,) and counts.is_contiguous()
+    dev = images[0].device
+    hw = torch.tensor([v for a in images for v in a.shape[:2]], dtype=torch.int32).pin_memory().to(dev, non_blocking=True)
+    src, dst = _ptr_table(images, dev), _ptr_table(outs, dev)
+    _lib.check(_lib.load().anysd_background_mask_u8(_ptr(src), _ptr(dst), _ptr(hw), B, max(a.shape[0] for a in images),
+                                                    max(a.shape[1] for a in images), _ptr(counts), _stream()), "background_mask")
+    _count()
+
+
 # ---- training step (SURVEY.md a24): thin wrappers, same conventions as above -------------------------------------
 def q_sample(x0, noise, t, sqrt_acp, sqrt_1m_acp, out):
     _cuda(x0, noise, t, out)

@@ -396,6 +396,34 @@ int anysd_clip_preprocess_plan(const int* hw, int B, int channels, int crop_mode
 int anysd_clip_preprocess_u8(const void* images, const void* table, int B, int patch, int rows_per_cta, int smem_bytes, const void* lut,
                              void* rows, void* crop_u8, anysd_stream_t stream);
 int anysd_l1_wrapped_u8(const void* a, const void* b, const void* nbytes, int B, long long max_bytes, void* out, anysd_stream_t stream);
+/* ---- inpainting edits (local_pipeline_tool.py background_change / replace, StableDiffusionInpaintPipeline) ----------------
+ * anysd_pil_resize_plan (host only): Image.resize of B whole images of any sizes, sizes = int [B, 4] (H, W, OH, OW), one filter
+ * per image (PIL_RESAMPLE_*: Pillow's enum; MODE1 is a mode "1" image given as 0/1 bytes -- other byte values are outside the
+ * contract -- NEAREST, then convert("L"), 0 / 255).  A band of at least one output row needs its source rows x OW x channels
+ * bytes of shared memory (at most 200 KB): an RGB LANCZOS upscale is limited to OW of about 9 500, EUNSUPPORTED beyond.
+ * The table holds per image a row of PIL_RESIZE_G = (H, W, OH, OW, x entries offset, x stride, y entries offset, y stride) and
+ * the entries; table = NULL sizes it (*table_ints).  *rows_per_cta, *smem_bytes and *bands (the grid's first extent) are the
+ * launch shape of anysd_pil_resize_u8, which takes device tables of B source and B destination pointers (uint8 HWC, channels
+ * 1 or 3 for the whole batch) and the table on the device; the bytes equal Pillow's.
+ * anysd_inpaint_prepare: uint8 img [B, H, W, 3] and mask [B, H, W] (H, W multiples of 8) -> masked_f16 [B, H, W, ldc]
+ * (channels 0..2 = fp16((byte / 255 * 2 - 1) * (mask < 128)), float32 as diffusers computes it; the rest 0), mask_latent fp32
+ * [B, 1, H / 8, W / 8] = (mask[8i, 8j] >= 128) and counts int32 [B] = the number of mask bytes >= 128.
+ * anysd_background_mask_u8: per image b of hw = int [B, 2] (H, W), the BGR uint8 [H, W, 3] at src[b] -> dst[b] uint8 [H, W] =
+ * (cvtColor(GaussianBlur(img, (5, 5), 0), BGR2GRAY) == 0), bit for bit OpenCV's; counts int32 [B] = its ones. */
+#define PIL_RESIZE_G 8
+#define PIL_RESAMPLE_NEAREST 0
+#define PIL_RESAMPLE_LANCZOS 1
+#define PIL_RESAMPLE_BICUBIC 3
+#define PIL_RESAMPLE_MODE1 16
+int anysd_pil_resize_plan(const int* sizes, const int* filters, int B, int channels, int* table, long long* table_ints, int* rows_per_cta,
+                          int* smem_bytes, int* bands);
+int anysd_pil_resize_u8(const void* src, const void* dst, const void* table, int B, int channels, int rows_per_cta, int smem_bytes,
+                        int bands, anysd_stream_t stream);
+int anysd_inpaint_prepare(const void* img, const void* mask, int B, int H, int W, int ldc, void* masked_f16, float* mask_latent,
+                          int* counts, anysd_stream_t stream);
+int anysd_background_mask_u8(const void* src, const void* dst, const void* hw, int B, int max_h, int max_w, int* counts,
+                             anysd_stream_t stream);
+
 int anysd_postfilter_scores_f32(const float* img_h, const float* txt_h, int E1, float logit_scale, const float* img_a, const float* img_b,
                                 const float* txt_a, const float* txt_b, int E2, int B, float* out, anysd_stream_t stream);
 
